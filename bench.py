@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Headline benchmark (BASELINE.json): EP dispatch+combine at EP=N on N B200s of one node, the
+"""Headline benchmark (BASELINE.json): EP dispatch+combine at EP=N on N H100s of one node, the
 reference's DeepEP-intranode config (4096 tokens/rank, hidden 7168, top-8 of 256 experts,
 bf16 -> fp8 dispatch, bf16 combine), plus an AllReduce bus-bandwidth sweep next to NCCL.
 
-Contract (driver):  python bench.py --gpus N --steps K --warmup W   (torchrun for N > 1)
+Usage:  python bench.py --gpus N --steps K --warmup W [--dump-outputs DIR]   (torchrun for N > 1)
 prints ONE JSON line on rank 0.  `value` = whole-job tokens/s through dispatch+combine
 (weak scaling: 4096 tokens per GPU), device-timed with CUDA events, max over ranks.
 
@@ -21,13 +21,13 @@ import os
 import statistics
 import sys
 import threading
-import time
 
 os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-BASELINE_DISPATCH_US = 571.0  # ep/README.md:154-160 (8xB200, EP=8, FP8 dispatch)
-BASELINE_COMBINE_US = 727.0   # ep/README.md:160     (8xB200, EP=8, BF16 combine)
+BASELINE_DISPATCH_US = 500.0  # the reference's ep/README.md, intranode (8xH200, EP=8, FP8 dispatch)
+BASELINE_COMBINE_US = 973.0   # the reference's ep/README.md, intranode (8xH200, EP=8, BF16 combine)
+DUMP_BYTES = 60 << 20         # cap of what --dump-outputs writes (a seeded sample of rows when the outputs are larger)
 
 
 def parse_args():
@@ -43,10 +43,12 @@ def parse_args():
     p.add_argument("--topk", type=int, default=8)
     p.add_argument("--experts", type=int, default=256)
     p.add_argument("--num-sms", type=int, default=int(os.environ.get("UCCL_B200_EP_SMS", "0")),
-                   help="CTAs per EP kernel of the headline (0: 148 at 1 GPU, else 24 = the reference's budget)")
+                   help="CTAs per EP kernel of the headline (0: every SM at 1 GPU, else 24 = the reference's budget)")
     p.add_argument("--no-allreduce-sweep", action="store_true")
     p.add_argument("--no-sm-sweep", action="store_true", help="only time the headline SM budget")
     p.add_argument("--out", default=None, help="also write the JSON line to this file")
+    p.add_argument("--dump-outputs", default=None, metavar="DIR",
+                   help="write the arrays the last timed step returned (rank 0) as DIR/<name>.npy")
     return p.parse_args()
 
 
@@ -113,15 +115,15 @@ class ClockSampler:
 
 # --------------------------------------------------------------------------- reference
 def run_reference(args):
-    """The unmodified reference from baseline/_ref through its own public API.  For the EP
+    """The unmodified reference from oracle/_ref through its own public API.  For the EP
     metric that is `uccl.ep.Buffer`, a native module the offline install cannot build (needs
     nanobind + libibverbs headers + its docker toolchain) -- see DESIGN.md."""
-    ref = os.path.join(os.path.dirname(os.path.abspath(__file__)), "baseline", "_ref")
+    ref = os.path.join(os.path.dirname(os.path.abspath(__file__)), "oracle", "_ref")
     rank = int(os.environ.get("RANK", "0"))
     if args.metric == "ep":
         why = None
         if not os.path.isdir(os.path.join(ref, "uccl")):
-            why = "baseline/_ref/uccl not installed"
+            why = "oracle/_ref/uccl not installed"
         else:
             sys.path.insert(0, ref)
             try:
@@ -138,7 +140,7 @@ def run_reference(args):
                 why = f"uccl.ep imported but its intranode bench failed: {type(e).__name__}: {e}"
         out = {"impl": "reference", "unavailable": why[:300]}
         # labelled DIAGNOSTIC (not the reference arm): the upstream DeepEP kernels the reference vendors and
-        # re-hosts as its intranode path, built from baseline/_ref/deepep, same config, num_sms = 24
+        # re-hosts as its intranode path, built from oracle/_ref/deepep, same config, num_sms = 24
         diag = None
         if args.gpus >= 2:
             # watchdog: a diagnostic must never hang the reference arm (the JSON line above is what the driver needs)
@@ -232,7 +234,6 @@ def run_reference_ep(args, ref):
     import torch.distributed as dist
 
     sys.path.insert(0, os.path.join(ref, "uccl", "ep_bench"))
-    sys.path.insert(0, os.path.join("/root/reference", "ep", "bench"))
     from buffer import Buffer as RefBuffer  # type: ignore
     from utils import per_token_cast_to_fp8 as ref_cast  # type: ignore
 
@@ -349,8 +350,10 @@ def main():
     # SM budget of the headline: the reference publishes its numbers at 24 SMs (ep/bench/test_intranode.py:571)
     # so that expert GEMMs can run beside the communication kernels -- the same budget is the default here for
     # N > 1 (like for like); other budgets are measured too and reported under "sm_sweep" / "best".  At N = 1
-    # nothing crosses NVLink (a pure HBM permutation) and the whole GPU is used.
-    head_sms = args.num_sms if args.num_sms > 0 else (148 if n == 1 else 24)
+    # nothing crosses NVLink (a pure HBM permutation) and the whole GPU is used: one CTA per SM, because the
+    # TMA pipelines fill an SM's shared memory and more CTAs than SMs would run in two waves.
+    head_sms = args.num_sms if args.num_sms > 0 else (torch.cuda.get_device_properties(dev).multi_processor_count
+                                                      if n == 1 else 24)
     cfg = Config(head_sms)
 
     def barrier():
@@ -401,7 +404,9 @@ def main():
         dist.all_reduce(verified, op=dist.ReduceOp.MIN)
     assert int(verified.item()) == 1, f"EP dispatch/combine verification failed on rank {rank}: bf16 {ok_bf16}, fp8 {ok_fp8}"
     comb_in = buf.get_combine_buffer(num_recv, H, K)
-    comb_in.normal_()  # stand-in for the expert MLP output (bf16), lives in the symmetric arena
+    # stand-in for the expert MLP output (bf16), lives in the symmetric arena; seeded so that every run combines
+    # the same values
+    comb_in.normal_(generator=torch.Generator(device=dev).manual_seed(4321 + rank))
     barrier()
 
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
@@ -412,7 +417,8 @@ def main():
 
     def measure(num_sms: int, steps: int, warm: int, sample_clocks: bool = False):
         """Times `steps` (dispatch + combine) steps at one SM budget: CUDA events around every step on the
-        launching stream, 256 MiB L2 flush write between steps (untimed), max over ranks."""
+        launching stream, 256 MiB L2 flush write between steps (untimed), max over ranks.  Also returns what the
+        last step gave back to the caller: (dispatched fp8 rows, their scales, combined rows)."""
         c = Config(num_sms)
 
         def step_cached():
@@ -426,15 +432,17 @@ def main():
         # capture dispatch and combine into CUDA graphs so the timed region measures the GPU, not the
         # interpreter (the kernels keep their cross-rank epochs on the device, so replays are safe).
         graphs = None
+        outs = None
         per_step_launches = 2
         if not args.no_graph:
             try:
                 l_before = launches()
                 g_d, g_c = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g_d):
-                    buf.dispatch(x, handle=handle, use_fp8=True, config=c)
+                    d_out = buf.dispatch(x, handle=handle, use_fp8=True, config=c)
                 with torch.cuda.graph(g_c):
-                    buf.combine(comb_in, handle, config=c)
+                    c_out = buf.combine(comb_in, handle, config=c)
+                outs = (d_out, c_out)  # a replay rewrites these tensors in place
                 per_step_launches = launches() - l_before
                 graphs = (g_d, g_c)
             except Exception as exc:  # pragma: no cover - fall back to eager launches
@@ -457,6 +465,10 @@ def main():
         starts = [torch.cuda.Event(enable_timing=True) for _ in range(steps)]
         mids = [torch.cuda.Event(enable_timing=True) for _ in range(steps)]
         ends = [torch.cuda.Event(enable_timing=True) for _ in range(steps)]
+        # Enqueuing a step costs the host more than the GPU needs to run it (flush + dispatch + combine), so a GPU fed
+        # step by step would idle inside the timed events waiting for the next launch.  A device-side sleep in front
+        # lets the host queue the timed steps ahead of the GPU: the events then time GPU work only.
+        torch.cuda._sleep(int(steps * (0.4e-3 if graphs is not None else 2e-3) * 2e9))  # cycles at <= 2 GHz
         # The host-side barrier above releases the ranks up to ~1 ms apart; without re-aligning the GPUs the
         # first timed dispatch would absorb that skew in its cross-rank entry barrier.  A device-side
         # barrier kernel (untimed) lines the GPUs up to within microseconds.
@@ -464,7 +476,6 @@ def main():
         l0 = launches()
         if sampler:
             sampler.start()
-        wall0 = time.perf_counter()
         for i in range(steps):
             flush.zero_()
             starts[i].record()
@@ -473,12 +484,13 @@ def main():
                 mids[i].record()
                 graphs[1].replay()
             else:
-                buf.dispatch(x, handle=handle, use_fp8=True, config=c)
+                d_out = buf.dispatch(x, handle=handle, use_fp8=True, config=c)
                 mids[i].record()
-                buf.combine(comb_in, handle, config=c)
+                c_out = buf.combine(comb_in, handle, config=c)
+                outs = (d_out, c_out)
             ends[i].record()
         barrier()
-        wall = time.perf_counter() - wall0
+        wall = starts[0].elapsed_time(ends[-1]) * 1e-3  # first step's start to last step's end, on the device
         clocks = sampler.stop() if sampler else None
         step_ms = [s.elapsed_time(e) for s, e in zip(starts, ends)]
         r = {
@@ -496,10 +508,13 @@ def main():
             "wall_s": wall, "clocks": clocks,
         }
         r["tokens_per_s"] = n * T / (r["ms_per_step"] * 1e-3)
-        return r
+        (q, sc), *_ = outs[0]
+        return r, (q[:num_recv], sc[:num_recv], outs[1][0])
 
     # ---- timed region of the headline: exactly K steps after W warm-up steps
-    head = measure(head_sms, args.steps, max(args.warmup, 3), sample_clocks=True)
+    head, head_out = measure(head_sms, args.steps, max(args.warmup, 3), sample_clocks=True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, head_out)  # before the sweep below reuses the arena
     ms_per_step, disp_ms, comb_ms = head["ms_per_step"], head["dispatch_us"] * 1e-3, head["combine_us"] * 1e-3
     tokens_per_s = head["tokens_per_s"]
     clocks, gpu_launches, wall, step_ms_stats = head["clocks"], head["gpu_launches"], head["wall_s"], head["step_us_min_med_max"]
@@ -509,14 +524,13 @@ def main():
     if not args.no_sm_sweep:
         for sms in ([24, 48, 96] if n > 1 else [24, 64]):
             if sms != head_sms:
-                sweep_rows.append(measure(sms, max(5, min(args.steps, 10)), 3))
+                sweep_rows.append(measure(sms, args.steps, 3)[0])
     best = max(sweep_rows, key=lambda r: r["tokens_per_s"])
 
     disp_bytes = num_recv * (H + H // 128 * 4)   # fp8 payload + scales received per rank
     comb_bytes = num_recv * H * 2                # bf16 rows pulled per rank
     remote_frac = (n - 1) / n
-    nvlink_gbs = 770.0   # measured one-direction peer-copy bandwidth on this pool (B200_PROFILING.md)
-    nvlink_nominal = 900.0
+    nvlink_nominal = 450.0  # NVLink 4 of an H100 SXM, one direction (data sheet)
 
     # ---- end-to-end through the public API, inputs from pinned host memory every step
     # Inputs of step i+1 are copied on a side stream while step i runs (every step still copies its
@@ -561,7 +575,7 @@ def main():
 
     run_e2e(3)
     barrier()
-    e2e_steps = max(3, min(args.steps, 10))
+    e2e_steps = args.steps
     s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     s.record()
     res = run_e2e(e2e_steps)
@@ -591,21 +605,19 @@ def main():
             "num_experts": E, "parallelism": f"ep{n}", "dispatch": "bf16 -> fused e4m3 + per-128 scales",
             "combine": "bf16", "num_sms": head_sms, "kernels": head["kernels"],
             "handle": "cached (as the reference times it)", "launch": graphs_used,
-            "l2": "256 MiB flush write between timed steps (untimed); per-step working set > 126 MB L2",
+            "l2": "256 MiB flush write between timed steps (untimed); per-step working set > 50 MB L2",
         },
         "dispatch_us": disp_ms * 1e3,
         "combine_us": comb_ms * 1e3,
         "dispatch_recv_GBps": disp_bytes / (disp_ms * 1e-3) / 1e9,
         "combine_recv_GBps": comb_bytes / (comb_ms * 1e-3) / 1e9,
-        # roofline: bytes that must cross NVLink / link bandwidth (measured 770 GB/s/dir peer copy; 900 nominal)
+        # roofline: bytes that must cross NVLink over the nominal link bandwidth (450 GB/s per direction)
         "roofline": {
-            "nvlink_GBps_measured": nvlink_gbs, "nvlink_GBps_nominal": nvlink_nominal,
+            "nvlink_GBps_nominal": nvlink_nominal,
             "dispatch_nvlink_GBps": disp_bytes * remote_frac / (disp_ms * 1e-3) / 1e9 if n > 1 else None,
             "combine_nvlink_GBps": comb_bytes * remote_frac / (comb_ms * 1e-3) / 1e9 if n > 1 else None,
-            "dispatch_floor_us": disp_bytes * remote_frac / (nvlink_gbs * 1e9) * 1e6 if n > 1 else None,
-            "combine_floor_us": comb_bytes * remote_frac / (nvlink_gbs * 1e9) * 1e6 if n > 1 else None,
-            "dispatch_frac_of_measured": (disp_bytes * remote_frac / (nvlink_gbs * 1e9)) / (disp_ms * 1e-3) if n > 1 else None,
-            "combine_frac_of_measured": (comb_bytes * remote_frac / (nvlink_gbs * 1e9)) / (comb_ms * 1e-3) if n > 1 else None,
+            "dispatch_floor_us": disp_bytes * remote_frac / (nvlink_nominal * 1e9) * 1e6 if n > 1 else None,
+            "combine_floor_us": comb_bytes * remote_frac / (nvlink_nominal * 1e9) * 1e6 if n > 1 else None,
             "dispatch_frac_of_nominal": (disp_bytes * remote_frac / (nvlink_nominal * 1e9)) / (disp_ms * 1e-3) if n > 1 else None,
             "combine_frac_of_nominal": (comb_bytes * remote_frac / (nvlink_nominal * 1e9)) / (comb_ms * 1e-3) if n > 1 else None,
             "hbm_GBps_single_gpu": ((T * H * 2 + disp_bytes) / (disp_ms * 1e-3) / 1e9) if n == 1 else None,
@@ -642,6 +654,24 @@ def main():
     if dist is not None:
         dist.destroy_process_group()
     return 0
+
+
+def dump_outputs(path, outs):
+    """Writes the dispatched e4m3 rows, their per-128-channel scales and the combined bf16 rows as float32 .npy
+    files, at most DUMP_BYTES in all: when the full arrays are larger, every array keeps the same seeded sample
+    of rows, so that two builds can be compared output for output."""
+    import numpy as np
+    import torch
+
+    os.makedirs(path, exist_ok=True)
+    row_bytes = sum(t[0].numel() * 4 for t in outs)
+    keep = max(1, DUMP_BYTES // row_bytes)
+    for name, t in zip(("dispatch_x", "dispatch_scales", "combine_x"), outs):
+        t = t.float()
+        if t.size(0) > keep:
+            rows = torch.randperm(t.size(0), generator=torch.Generator().manual_seed(0))[:keep].sort().values
+            t = t[rows.to(t.device)]
+        np.save(os.path.join(path, name + ".npy"), t.cpu().numpy())
 
 
 def allreduce_sweep(comm, dist, dev, n, max_over_ranks, barrier):

@@ -37,7 +37,7 @@ def main():
     dist.init_process_group("cpu:gloo,cuda:nccl", device_id=dev)
     dt = {"bf16": torch.bfloat16, "fp32": torch.float32, "fp16": torch.float16}[args.dtype]
     es = torch.empty((), dtype=dt).element_size()
-    comm = Communicator.from_torch_dist(heap_bytes=(6 << 30), stage_bytes=256 << 20, max_ctas=148)
+    comm = Communicator.from_torch_dist(heap_bytes=(6 << 30), stage_bytes=256 << 20, max_ctas=132)
     n = world
     big_in = comm.empty(args.max // es, dtype=dt)
     big_out = comm.empty(args.max // es, dtype=dt)

@@ -21,7 +21,7 @@ def main():
     p = Proxy(comm, capacity=a.capacity)
     res = {"capacity": a.capacity, "throughput": [], "latency_us": None}
     with torch.cuda.device(comm.device):
-        for blocks, threads in ((1, 32), (1, 256), (8, 256), (32, 256), (148, 256)):
+        for blocks, threads in ((1, 32), (1, 256), (8, 256), (32, 256), (132, 256)):
             p.bench_throughput(blocks, threads, 16)  # warm-up
             r = p.bench_throughput(blocks, threads, 64)
             res["throughput"].append({"blocks": blocks, "threads": threads, "mcmd_per_s": r / 1e6})

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Same-box anchor: the UPSTREAM DeepEP intranode kernels vendored by the reference
-(/root/reference/thirdparty/DeepEP, unmodified sources, its own setup.py with the DISABLE_NVSHMEM branch,
-built for sm_100 into baseline/_ref/deepep by scripts/build_deepep_baseline.sh) on the headline config.
+(thirdparty/DeepEP of the reference, unmodified sources, its own setup.py with the DISABLE_NVSHMEM branch,
+built for sm_90a into oracle/_ref/deepep by oracle/build_deepep.sh) on the headline config.
 
 The reference's own `uccl.ep` cannot be built offline (nanobind + libibverbs headers are absent), but its
 intranode dispatch/combine kernels are DeepEP's re-hosted (SURVEY.md section 0, fact 5; ep/src/intranode.cu),
@@ -24,13 +24,13 @@ import os
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DEEPEP_DIR = os.path.join(ROOT, "baseline", "_ref", "deepep")
+DEEPEP_DIR = os.path.join(ROOT, "oracle", "_ref", "deepep")
 
 
 def available() -> str | None:
     """None if the vendored DeepEP build is importable, else the reason."""
     if not os.path.isdir(os.path.join(DEEPEP_DIR, "deep_ep")):
-        return "baseline/_ref/deepep not built (scripts/build_deepep_baseline.sh)"
+        return "oracle/_ref/deepep not built (oracle/build_deepep.sh)"
     return None
 
 
@@ -117,7 +117,7 @@ def run(tokens=4096, hidden=7168, topk=8, experts=256, num_sms=24, iters=20, war
         rows["combine_bf16"][str(ch) if ch else "default"] = timed(lambda: buffer.combine(x=recv_x, handle=handle, config=cfg))
     best = {k: min(v.values()) for k, v in rows.items()}
     out = {
-        "what": "upstream DeepEP (reference/thirdparty/DeepEP, unmodified, DISABLE_NVSHMEM, sm_100) intranode kernels",
+        "what": "upstream DeepEP (reference/thirdparty/DeepEP, unmodified, DISABLE_NVSHMEM, sm_90a) intranode kernels",
         "n_gpus": n, "tokens": T, "hidden": H, "topk": K, "experts": E, "num_sms": num_sms,
         "num_recv_tokens": num_recv, "iters": iters, "timing": "CUDA events, 256 MiB L2 flush per call, max over ranks",
         "fp8_cast_torch_us": cast_us, "layout_us": layout_us,

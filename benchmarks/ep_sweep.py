@@ -23,7 +23,7 @@ def main():
     p.add_argument("--hidden", type=int, default=7168)
     p.add_argument("--topk", type=int, default=8)
     p.add_argument("--experts", type=int, default=256)
-    p.add_argument("--sms", default="16,24,32,48,64,96,128,148")
+    p.add_argument("--sms", default="16,24,32,48,64,96,128,132")
     p.add_argument("--iters", type=int, default=20)
     p.add_argument("--impls", default="reg,tma", help="kernel implementations to sweep: reg (register path), tma (TMA pipelines)")
     p.add_argument("--modes", default="fp8_fused,bf16")

@@ -37,7 +37,7 @@ def main():
     idx = (torch.randn(T, E, generator=g).abs() + 1).topk(K, dim=-1).indices.to(torch.int64).contiguous().cuda()
     w = torch.rand(T, K, generator=g).float().cuda()
     for _ in range(a.reps):
-        for impl, sms in ((C.EP_IMPL_REG, 148), (C.EP_IMPL_TMA, 148), (C.EP_IMPL_TMA, 24), (C.EP_IMPL_REG, 24)):
+        for impl, sms in ((C.EP_IMPL_REG, 132), (C.EP_IMPL_TMA, 132), (C.EP_IMPL_TMA, 24), (C.EP_IMPL_REG, 24)):
             buf.runtime.impl = impl
             cfg = Config(sms)
             tpr, _, tpe, in_rank, _ = buf.get_dispatch_layout(idx, E)

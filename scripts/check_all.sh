@@ -1,6 +1,6 @@
 #!/usr/bin/env bash
 # Everything that can be checked without a GPU, in the order the CI runs it:
-#   build for sm_100a -> CPU test-suite -> transport under ASan/UBSan and TSan -> GPU tests only collected.
+#   build for sm_90a -> CPU test-suite -> transport under ASan/UBSan and TSan -> GPU tests only collected.
 # With --profiles the CPU-side scale-out measurements under profiles/ are regenerated as well.
 set -euo pipefail
 ROOT="$(cd "$(dirname "$0")/.." && pwd)"

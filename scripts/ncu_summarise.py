@@ -64,7 +64,7 @@ def main():
                         w.writerow([k, r[col[k]]])
             table.append((key, vals))
     with open(os.path.join(root, "profiles", "NCU_SUMMARY.md"), "w") as f:
-        f.write("# ncu --set full summaries (1 B200, one-rank communicator, benchmarks/ncu_targets.py)\n\n")
+        f.write("# ncu --set full summaries (1 H100, one-rank communicator, benchmarks/ncu_targets.py)\n\n")
         f.write("Durations under ncu are serialised and cold-cache: compare shares and percentages, not absolutes.\n\n")
         f.write("| kernel@grid | us | regs | warps active % | DRAM % of peak | DRAM read MB | DRAM write MB | long-scoreboard stall % | barrier stall % |\n")
         f.write("|---|---:|---:|---:|---:|---:|---:|---:|---:|\n")

@@ -3,9 +3,9 @@
 with the committed baseline of the same GPU count in profiles/ and fails when a tracked number got worse by more
 than the tolerance.  The reference has no automated perf regression check (SURVEY 4: "numbers are pasted into READMEs").
 
-    python bench.py --gpus 8 ... > new8.json
-    python scripts/perf_gate.py new8.json                      # baseline: profiles/bench8.json, tolerance 7 %
-    python scripts/perf_gate.py new8.json --baseline old.json --tolerance 0.05 --update
+    python bench.py --gpus 1 ... > new1.json
+    python scripts/perf_gate.py new1.json                      # baseline: profiles/bench1.json, tolerance 7 %
+    python scripts/perf_gate.py new1.json --baseline old.json --tolerance 0.05 --update
 """
 import argparse
 import json

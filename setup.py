@@ -1,4 +1,4 @@
-"""Builds the native core in-tree (nvcc -gencode arch=compute_100a,code=sm_100a) before packaging.
+"""Builds the native core in-tree (nvcc -gencode arch=compute_90a,code=sm_90a) before packaging.
 `pip install -e .` / `python setup.py build_ext --inplace` both end up in uccl_b200/_build.py, the same
 entry point `__graft_entry__.build()` uses."""
 import importlib.util

@@ -1,5 +1,8 @@
-"""Shared helpers for the GPU tests: virtual ranks on one device (or real devices when the
-box has enough of them)."""
+"""Shared helpers for the tests: virtual ranks on one device (or real devices when the box has enough of
+them), and the stored call signatures of the reference project."""
+import functools
+import json
+import os
 import threading
 
 import torch
@@ -7,6 +10,14 @@ import torch
 from uccl_b200 import Communicator
 
 _WORLDS = {}
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+
+
+@functools.lru_cache(maxsize=None)
+def reference_signatures():
+    """Parameter names of the reference project's public Python / binding API (oracle/extract_signatures.py)."""
+    with open(os.path.join(GOLDEN, "reference_signatures.json")) as f:
+        return json.load(f)
 
 
 def devices_for(n):

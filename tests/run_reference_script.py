@@ -1,5 +1,6 @@
 """Runs a script written against the reference's ``uccl`` package on this library: installs the module aliases
-(`uccl_b200.compat`) and executes the script as ``__main__``.  Used by tests/test_reference_scripts.py.
+(`uccl_b200.compat`) and executes the script as ``__main__``.  A manual tool: run it on
+scripts from a checkout of the reference (the test-suite does not run them).
 
     python tests/run_reference_script.py /path/to/reference/p2p/tests/test_engine_send.py [args...]
 """

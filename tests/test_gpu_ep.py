@@ -18,7 +18,7 @@ def get_buffers(n, nbytes=192 << 20):
     if n not in _BUFFERS:
         comms = get_world(n, heap_mb=256 + 224, stage_mb=8, max_ctas=4)
         _BUFFERS[n] = [Buffer(comm=c, num_nvl_bytes=nbytes) for c in comms]
-        # virtual ranks share one GPU: all n kernels must be co-resident (n * num_sms <= 148 SMs)
+        # virtual ranks share one GPU: all n kernels must be co-resident (n * num_sms <= 132 SMs)
         Buffer.set_num_sms(8)
     return _BUFFERS[n]
 

@@ -365,63 +365,47 @@ def test_ep_bootstrap_helpers():
 def test_buffer_signature_audit_against_the_reference_and_upstream_deepep():
     """Every public method of the reference's `Buffer` (ep/bench/buffer.py) and of the upstream DeepEP it vendors
     (thirdparty/DeepEP/deep_ep/buffer.py) exists here with the same parameter names (frameworks call them by keyword).
-    Skipped where the reference tree is not mounted."""
-    import ast
+    The reference's signatures are stored in tests/golden/reference_signatures.json (oracle/extract_signatures.py)."""
     import inspect
-    import os
 
     import deep_ep
+    from helpers import reference_signatures
     from uccl_b200.ep.buffer import Buffer as Native
     from uccl_b200.ep.low_latency import LowLatencyRuntime
 
-    files = ["/root/reference/ep/bench/buffer.py", "/root/reference/thirdparty/DeepEP/deep_ep/buffer.py",
-             "/root/reference/ep/deep_ep_wrapper/deep_ep/buffer.py"]
-    files = [f for f in files if os.path.exists(f)]
-    if not files:
-        pytest.skip("reference tree not available")
+    files = reference_signatures()["ep_buffer"]
+    assert len(files) == 3
     ll = {"low_latency_dispatch": LowLatencyRuntime.dispatch, "low_latency_combine": LowLatencyRuntime.combine}
     internal = {"connect_atomic_buffer"}  # takes the reference's own proxy type; checked by name only
-    for path in files:
-        tree = ast.parse(open(path).read())
-        cls = next(n for n in ast.walk(tree) if isinstance(n, ast.ClassDef) and n.name == "Buffer")
-        for f in cls.body:
-            if not isinstance(f, ast.FunctionDef) or (f.name.startswith("_") and f.name != "__init__"):
+    for path, methods in files.items():
+        for name, want in methods.items():
+            assert hasattr(deep_ep.Buffer, name) and hasattr(Native, name), f"{path}: Buffer.{name} missing"
+            if name in internal:
                 continue
-            assert hasattr(deep_ep.Buffer, f.name) and hasattr(Native, f.name), f"{path}: Buffer.{f.name} missing"
-            if f.name in internal:
-                continue
-            want = [a.arg for a in f.args.posonlyargs + f.args.args + f.args.kwonlyargs if a.arg != "self"]
-            target = ll.get(f.name, getattr(Native, f.name))
+            target = ll.get(name, getattr(Native, name))
             have = set(inspect.signature(target).parameters)
             missing = [w for w in want if w not in have]
-            assert not missing, f"{path}: Buffer.{f.name} lacks parameters {missing}"
+            assert not missing, f"{path}: Buffer.{name} lacks parameters {missing}"
 
 
 def test_utils_signature_audit_against_the_reference_helpers():
     """Every public helper of the reference's ep/bench/utils.py (what its tests and benchmarks import) and of
     upstream DeepEP's utils exists under `uccl_b200.ep` with the same parameter names."""
-    import ast
     import inspect
-    import os
 
     import uccl_b200.ep as E
     import uccl_b200.ep.utils as U
+    from helpers import reference_signatures
 
-    files = ["/root/reference/ep/bench/utils.py", "/root/reference/thirdparty/DeepEP/deep_ep/utils.py",
-             "/root/reference/thirdparty/DeepEP/tests/utils.py", "/root/reference/ep/deep_ep_wrapper/deep_ep/utils.py"]
-    files = [f for f in files if os.path.exists(f)]
-    if not files:
-        pytest.skip("reference tree not available")
-    for path in files:
-        for f in ast.parse(open(path).read()).body:
-            if not isinstance(f, ast.FunctionDef) or f.name.startswith("_"):
-                continue
-            target = getattr(U, f.name, None) or getattr(E, f.name, None)
-            assert target is not None, f"{path}: {f.name} missing"
-            want = [a.arg for a in f.args.posonlyargs + f.args.args + f.args.kwonlyargs]
+    files = reference_signatures()["ep_utils"]
+    assert len(files) == 4
+    for path, funcs in files.items():
+        for name, want in funcs.items():
+            target = getattr(U, name, None) or getattr(E, name, None)
+            assert target is not None, f"{path}: {name} missing"
             have = set(inspect.signature(target).parameters)
             missing = [w for w in want if w not in have]
-            assert not missing, f"{path}: {f.name} lacks parameters {missing}"
+            assert not missing, f"{path}: {name} lacks parameters {missing}"
 
 
 def test_per_token_cast_back_accepts_both_spellings():
@@ -600,17 +584,10 @@ def test_sglang_call_shapes_on_the_host_backend():
 
 
 def test_deep_ep_package_exports_what_the_reference_wrapper_exports():
-    import ast
-    import os
-
     import deep_ep
+    from helpers import reference_signatures
 
-    path = "/root/reference/ep/deep_ep_wrapper/deep_ep/__init__.py"
-    if not os.path.exists(path):
-        pytest.skip("reference tree not available")
-    for n in ast.walk(ast.parse(open(path).read())):
-        if isinstance(n, ast.Assign) and any(getattr(t, "id", "") == "__all__" for t in n.targets):
-            missing = [x for x in ast.literal_eval(n.value) if not hasattr(deep_ep, x)]
-            assert not missing, missing
-            return
-    raise AssertionError("no __all__ in the reference wrapper")
+    exported = reference_signatures()["deep_ep_all"]  # __all__ of the reference's ep/deep_ep_wrapper/deep_ep
+    assert exported
+    missing = [x for x in exported if not hasattr(deep_ep, x)]
+    assert not missing, missing

@@ -347,26 +347,17 @@ def test_engine_concurrency_stress_under_sanitizers(tmp_path, san):
 
 def test_endpoint_signature_audit_against_the_reference_binding():
     """Every method of the reference's nanobind `Endpoint` (p2p/engine_api.cc) exists with the same keyword names
-    (`nb::arg(...)`) in the same order.  Skipped where the reference tree is not mounted."""
+    (`nb::arg(...)`) in the same order.  The binding's argument lists are stored in
+    tests/golden/reference_signatures.json (oracle/extract_signatures.py)."""
     import inspect
-    import os
-    import re
 
+    from helpers import reference_signatures
     from uccl_b200 import p2p
     from uccl_b200.p2p import Endpoint
 
-    path = "/root/reference/p2p/engine_api.cc"
-    if not os.path.exists(path):
-        pytest.skip("reference tree not available")
-    src = open(path).read()
-    src = src[src.index('nb::class_<Endpoint>'):] if 'nb::class_<Endpoint>' in src else src
     checked = 0
-    for d in re.split(r'\.def\(\s*"', src)[1:]:
-        name = d.split('"', 1)[0]
-        if name.startswith("__"):
-            continue
+    for name, want in reference_signatures()["p2p_endpoint"].items():
         assert hasattr(Endpoint, name), f"Endpoint.{name} missing"
-        want = re.findall(r'nb::arg\("([a-zA-Z_0-9]+)"\)', d.split(".def(", 1)[0])
         if name == "get_metadata":
             continue  # the reference fills a caller-provided vector; here the bytes are returned
         have = [p for p in inspect.signature(getattr(Endpoint, name)).parameters if p != "self"]
@@ -385,33 +376,22 @@ def test_endpoint_signature_audit_against_the_reference_binding():
 
 def test_collective_signature_audit_against_the_reference():
     """Module functions and `CollectiveContext` methods of the reference's `uccl.collective` (p2p/collective.py) exist
-    here with the same parameter names."""
-    import ast
+    here with the same parameter names (stored in tests/golden/reference_signatures.json)."""
     import inspect
-    import os
 
     import uccl_b200.collective as c
+    from helpers import reference_signatures
 
-    path = "/root/reference/p2p/collective.py"
-    if not os.path.exists(path):
-        pytest.skip("reference tree not available")
-
-    def params(f):
-        a = f.args
-        return [x.arg for x in a.posonlyargs + a.args + a.kwonlyargs if x.arg != "self"]
-
+    ref = reference_signatures()["collective"]
     n = 0
-    for node in ast.parse(open(path).read()).body:
-        if isinstance(node, ast.FunctionDef) and not node.name.startswith("_"):
-            have = list(inspect.signature(getattr(c, node.name)).parameters)
-            assert not [p for p in params(node) if p not in have], (node.name, params(node), have)
-            n += 1
-        if isinstance(node, ast.ClassDef) and node.name == "CollectiveContext":
-            for f in node.body:
-                if isinstance(f, ast.FunctionDef) and (not f.name.startswith("_") or f.name == "__init__"):
-                    have = list(inspect.signature(getattr(c.CollectiveContext, f.name)).parameters)
-                    assert not [p for p in params(f) if p not in have], (f.name, params(f), have)
-                    n += 1
+    for name, want in ref["functions"].items():
+        have = list(inspect.signature(getattr(c, name)).parameters)
+        assert not [p for p in want if p not in have], (name, want, have)
+        n += 1
+    for name, want in ref["CollectiveContext"].items():
+        have = list(inspect.signature(getattr(c.CollectiveContext, name)).parameters)
+        assert not [p for p in want if p not in have], (name, want, have)
+        n += 1
     assert n > 25
 
 

@@ -1,4 +1,4 @@
-"""uccl_b200 -- a Blackwell-native (sm_100a, NVLink 5 / NVSwitch) GPU communication library
+"""uccl_b200 -- a Hopper-native (sm_90a, NVLink 4 / NVSwitch) GPU communication library
 with the capabilities of uccl-project/uccl:
 
 * ``uccl_b200.collective``  NCCL-style collectives (hand-written P2P / NVLS kernels over a

@@ -1,6 +1,6 @@
-"""In-tree native build: nvcc (sm_100a) for the kernels, host compiler for the runtime.
+"""In-tree native build: nvcc (sm_90a) for the kernels, host compiler for the runtime.
 
-Everything is compiled with ``-gencode arch=compute_100a,code=sm_100a -lineinfo`` and linked
+Everything is compiled with ``-gencode arch=compute_90a,code=sm_90a -lineinfo`` and linked
 into ``uccl_b200/_C.<abi>.so`` (pybind11 module) next to this file, so the shared object
 travels with the repo snapshot to the GPU box.  Incremental: an object is rebuilt when its
 source or any header under csrc/ is newer.
@@ -22,7 +22,7 @@ ROOT = Path(__file__).resolve().parent
 CSRC = ROOT / "csrc"
 BUILD = ROOT.parent / "build" / "obj"
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC = os.environ.get("NVCC", shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc")
 
 
@@ -94,7 +94,7 @@ def _compile_one(src: Path, obj: Path, verbose: bool) -> None:
 
 
 def build(force: bool = False, verbose: bool = False, jobs: int | None = None) -> Path:
-    """Compile every CUDA/C++ source for sm_100a and link the python module. Returns its path."""
+    """Compile every CUDA/C++ source for sm_90a and link the python module. Returns its path."""
     if not Path(NVCC).exists():
         raise RuntimeError(f"nvcc not found at {NVCC}")
     BUILD.mkdir(parents=True, exist_ok=True)

@@ -1,7 +1,7 @@
 """Loader of the native extension.
 
 The CUDA path must never silently degrade: if the shared object is missing it is built
-in-tree (nvcc, sm_100a); if that is impossible an ImportError with the build log is raised.
+in-tree (nvcc, sm_90a); if that is impossible an ImportError with the build log is raised.
 """
 from __future__ import annotations
 

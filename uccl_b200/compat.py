@@ -41,7 +41,7 @@ def install(name: str = "uccl") -> types.ModuleType:
 
     def _other_hardware(what):
         def f():
-            raise NotImplementedError(f"uccl_b200 is an sm_100a / NVLink library: there is no {what}")
+            raise NotImplementedError(f"uccl_b200 is an sm_90a / NVLink library: there is no {what}")
 
         return f
 

@@ -24,7 +24,7 @@ static inline cudaStream_t S(uintptr_t s) { return reinterpret_cast<cudaStream_t
 static inline void* P(uintptr_t p) { return reinterpret_cast<void*>(p); }
 
 PYBIND11_MODULE(_C, m) {
-  m.doc() = "uccl_b200 native core: symmetric-heap fabric, sm_100a collectives, EP, P2P engine";
+  m.doc() = "uccl_b200 native core: symmetric-heap fabric, sm_90a collectives, EP, P2P engine";
   m.attr("MAX_RANKS") = kMaxRanks;
   m.attr("LL_MAX_BYTES") = (uint64_t)kLLMaxData;
 

@@ -24,7 +24,7 @@ UB_PARAM(NvlsCtas, "NVLS_CTAS", 0)  // 0: 256 / nranks
 UB_PARAM(ForceKernels, "FORCE_KERNELS", 0)
 UB_PARAM(NvlsUnroll, "NVLS_UNROLL", 4)  // multimem.ld_reduce in flight per thread of twoshot_nvls (4 or 8)
 // plain (non-symmetric) buffers of at least this size take the block-pipelined staged kernel (needs NVLS, > 2 ranks)
-UB_PARAM(ArPipeMinBytes, "AR_PIPE_MIN_BYTES", 512 << 20)  // measured on 8 GPUs: wins at 1 GiB (2.50 vs 2.75 ms serial, 2.59 NCCL), loses at 256 MiB
+UB_PARAM(ArPipeMinBytes, "AR_PIPE_MIN_BYTES", 512 << 20)  // from 8-GPU sweeps of benchmarks/allreduce_perf.py: wins at 1 GiB, loses at 256 MiB
 
 const char* algo_name(int algo) {
   switch (algo) {
@@ -285,13 +285,12 @@ int Comm::select_allreduce(size_t bytes, bool symmetric, int dtype, int op, int*
     }
   }
   if (algo == ALGO_AUTO) {
-    // defaults measured on B200 (benchmarks/allreduce_perf.py, profiles/): the packet path wins
+    // defaults from benchmarks/allreduce_perf.py sweeps on NVSwitch boxes: the packet path wins
     // until its N-fold traffic outweighs the two barriers of the two-shot kernels
     uint64_t ll_max = (uint64_t)ubParamArLLMaxBytes();
-    // n = 2: the two barriers of the two-shot kernels cost ~20 us when both GPUs are driven by one host thread
-    // (nccl-tests -g 2: 35 us at 1 MiB vs 15 us for the packet path), so packets carry up to the 1 MiB cap there
-    // n = 4 (nccl-tests + bench on 4xB200): ordinary buffers at 512 KiB - 1 MiB take 26-30 us through the staged kernels
-    // vs 20-22 us for NCCL; the packet path has no barrier
+    // n = 2: the two barriers of the two-shot kernels dominate when both GPUs are driven by one host thread, so
+    // packets carry up to the 1 MiB cap there; n = 4: ordinary buffers of 512 KiB - 1 MiB are slower through the
+    // staged kernels than through NCCL, and the packet path has no barrier
     if (ll_max == 0) ll_max = n <= 4 ? (1u << 20) : (128u << 10);
     ll_max = std::min<uint64_t>(ll_max, kLLMaxData);
     // with 2 ranks the switch cannot reduce traffic (both paths move `size` per direction) and the
@@ -347,7 +346,7 @@ static cudaError_t launch_ar_any(int algo, int dtype, int op, int out_dtype, con
 // per-rank piece size up to which the barrier-free LL exchange kernels are used
 static uint64_t xchg_ll_limit(int64_t v, int n, bool symmetric_push) {
   if (v < 0) return 0;
-  uint64_t m = v > 0 ? (uint64_t)v : (n <= 4 ? (256u << 10) : (128u << 10));  // 4 ranks: reduce_scatter of 1 MiB was 30 vs 20 us (NCCL) staged
+  uint64_t m = v > 0 ? (uint64_t)v : (n <= 4 ? (256u << 10) : (128u << 10));  // 4 ranks: a staged 1 MiB reduce_scatter was slower than NCCL
   if (v == 0 && symmetric_push) m = 32u << 10;  // the push kernels only pay one barrier
   return std::min<uint64_t>(m, kLLMaxData);
 }
@@ -496,7 +495,7 @@ void Comm::allgather(const void* in, void* out, size_t count_per_rank, int dtype
   int ctas;
   const bool ll_mc = has_multicast() && n > 2;
   // with multicast one multimem.st publishes a packet to every peer, which keeps the LL path ahead
-  // of the barrier-based kernels up to 512 KiB pieces (measured on 8 GPUs: profiles/allgather8.json)
+  // of the barrier-based kernels up to 512 KiB pieces (8-GPU all-gather sweeps)
   uint64_t ag_ll_max = xchg_ll_limit(xchg_ll_max_, n, out_sym && !ll_mc);
   if (xchg_ll_max_ == 0 && ll_mc) ag_ll_max = std::min<uint64_t>(512u << 10, kLLMaxData);
   if (bytes % 16 == 0 && bytes <= ag_ll_max) {
@@ -551,8 +550,7 @@ void Comm::reduce_scatter(const void* in, void* out, size_t recv_count, int dtyp
   const bool in_sym = in_heap(in, bytes * n) && (bytes % 16 == 0);
   if (in_sym) a.in_off = heap_offset(in);
   // staged input: pushing pieces into the peers' stages wins except for very large messages on
-  // NVLS systems, where copy-in + multimem.ld_reduce is ahead (8 GPUs, 1 GiB: 1.74 ms vs 1.91 ms;
-  // 64 MiB: 171 us vs 160 us -- profiles/reduce_scatter8*.json)
+  // NVLS systems, where copy-in + multimem.ld_reduce is ahead (8-GPU reduce-scatter sweeps, from 256 MiB)
   const bool nvls_possible = has_multicast() && nvls_reduce_supported(dtype, op) && n > 2;
   a.variant = (rs_push_ && !(nvls_possible && bytes * (uint64_t)n >= (256ull << 20))) ? 1 : 0;
   const bool nvls = has_multicast() && nvls_reduce_supported(dtype, op) && n > 2;

@@ -1,6 +1,6 @@
 // NCCL-API drop-in: exports the nccl.h symbol set on top of the native communicator, so code
 // written against NCCL (nccl-tests style harnesses, frameworks that dlopen/LD_PRELOAD libnccl)
-// runs on the hand-written sm_100a kernels.
+// runs on the hand-written sm_90a kernels.
 //
 // Reference counterpart: experimental/lite/nccl/nccl.cu:1351-2430 (which falls back to a
 // dlopen'd NCCL for ReduceScatter/Reduce and leaves AllToAll(v)/PreMulSum/CommAbort as stubs).

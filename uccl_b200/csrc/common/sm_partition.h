@@ -1,7 +1,7 @@
 // SM partitions: a fixed set of SMs carved out of a GPU as a CUDA green context, plus streams bound to it.
 //
 // Why it exists here: the communication kernels of this library run on an SM budget (the expert-parallel kernels on
-// 24 of the 148 SMs, like the reference's DeepEP configuration), but a budget expressed as a grid size only limits how
+// 24 of the 132 SMs of an H100, like the reference's DeepEP configuration), but a budget expressed as a grid size only limits how
 // many CTAs the kernel brings -- not WHERE they land, and a GEMM launched first can leave them queued behind its waves.
 // A partition makes the budget physical: kernels launched on a partition's stream only ever occupy that partition's
 // SMs, and the complementary partition keeps compute off them.  The reference probes the same mechanism as a

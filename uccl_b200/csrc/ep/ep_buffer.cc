@@ -88,16 +88,14 @@ void EpBuffer::set_impl(int impl) {
   impl_ = impl;
 }
 
-// Measured (profiles/ep_sweep_{2,8}xB200.json): across NVLink the TMA pipelines match the register path on
-// dispatch at every SM budget and win the combine by 5-10 % (458 vs 511 us at 24 SMs, 436 vs 461 us at 96 on
-// 8 GPUs); on ONE GPU (HBM-only permutation, nothing to hide) the register path's shorter per-token critical
-// path is faster (29 vs 37 us combine at 148 CTAs).
+// Across NVLink the TMA pipelines keep more bytes in flight per CTA than the register path; on ONE GPU (HBM-only
+// permutation, nothing to hide) the register path's shorter per-token critical path is faster
+// (benchmarks/ep_sweep.py times both).
 int EpBuffer::pick_impl(int grid, bool combine) const {
   if (impl_ != EP_IMPL_AUTO) return impl_;
   if (nranks() == 1) return EP_IMPL_REG;
   // 2 GPUs, few CTAs: a token has two copies and one of them is local, so combine is bound by a CTA's own critical
-  // path, not by bytes in flight -- the register path wins there (24 CTAs: 166 vs 201 us; 48 CTAs: 118 vs 113 us,
-  // profiles/ep_sweep_2xB200.json); dispatch favours the pipelines at every CTA count (119 vs 136 us at 24)
+  // path, not by bytes in flight -- the register path wins there; dispatch favours the pipelines at every CTA count
   if (combine && nranks() == 2 && grid <= 32) return EP_IMPL_REG;
   return EP_IMPL_TMA;
 }

@@ -1,4 +1,4 @@
-// Host runtime of the expert-parallel buffer (B200-native counterpart of the reference's
+// Host runtime of the expert-parallel buffer (Hopper-native counterpart of the reference's
 // `class Buffer`, ep/src/uccl_ep.cc:315-1600).  No IPC-handle exchange, proxies or ring
 // buffers: the buffer is one block of the communicator's symmetric heap carved into
 //   [ctrl | dispatch arena 0 .. S-1 | combine arena]

@@ -1,11 +1,11 @@
-// Expert-parallel dispatch / combine kernels for one NVSwitch node (sm_100a).
+// Expert-parallel dispatch / combine kernels for one NVSwitch node (sm_90a).
 //
 // What the reference does (ep/src/layout.cu:9-150, ep/src/intranode.cu:12-1152): a layout
 // kernel, a notify kernel that all-to-alls the counts, then sender CTAs copy tokens into the
 // *receiver's ring buffer* and receiver CTAs copy them again into recv_x (two passes over the
 // payload, FP8 cast done beforehand by separate torch kernels, ep/bench/utils.py:666-675).
 //
-// B200-native design here -- direct placement, one pass, fused cast:
+// Hopper-native design here -- direct placement, one pass, fused cast:
 //   * counts are exchanged inside the dispatch kernel (peer stores + block barrier), every rank
 //     then knows the full R x R matrix and therefore the exact slot of each of its tokens in each
 //     destination arena: no ring, no receiver CTAs, no second copy;
@@ -91,7 +91,7 @@ __global__ void __launch_bounds__(1024, 1) ep_layout_kernel(const EpLayoutArgs a
 // CTAs (they were scheduled earlier, so the wait cannot deadlock even if the grid is not co-resident)
 // and then writes the same stable positions as the single-CTA kernel.  The expert histogram is
 // accumulated in shared memory and added to the global one, which CTA 0 zeroes before it publishes.
-// Replaces a 22 us single-CTA scan (40 % of an EP=1 step) with ~4 us.
+// Replaces a single-CTA scan that took a large share of an EP=1 step.
 __global__ void __launch_bounds__(kEpLayoutThreads) ep_layout_mc_kernel(const EpLayoutArgs a) {
   extern __shared__ int s_dyn[];
   int* s_expert = s_dyn;                                               // [E]
@@ -256,7 +256,7 @@ __global__ void __launch_bounds__(512, 1) ep_dispatch_kernel(const __grid_consta
 
       if constexpr (MODE == EP_X_FUSED_FP8) {
         const int units = a.H / 16;  // 16 output bytes (16 channels) per lane-iteration
-        constexpr int PF = 4;        // iterations whose loads are in flight together (8 x 16 B per lane; 7 was not faster at 148 CTAs and spills)
+        constexpr int PF = 4;        // iterations whose loads are in flight together (8 x 16 B per lane; 7 spills)
         for (int ub = 0; ub < units; ub += 32 * PF) {
           uint4 v0[PF], v1[PF];
 #pragma unroll

@@ -1,4 +1,4 @@
-// Low-latency (decode) expert-parallel kernels, sm_100a.
+// Low-latency (decode) expert-parallel kernels, sm_90a.
 //
 // Reference behaviour (ep/src/internode_ll.cu:50-731, 735-1304): dispatch casts each token to
 // fp8, atomically claims a slot per (expert, source-rank) region at the destination, stores the
@@ -6,7 +6,7 @@
 // regions into the contiguous per-expert layout; combine pushes expert outputs back into a
 // [token][topk] staging area at the source and a RECV phase does the weighted reduction.
 //
-// B200-native design: ONE pass each way.
+// Hopper-native design: ONE pass each way.
 //   dispatch: every rank all-gathers its per-expert histogram first (E ints to each peer + one
 //     block barrier), so each sender knows the exact packed offset of its tokens inside every
 //     remote expert's contiguous block.  A warp stages the (fp8-cast) token + scales in shared

@@ -1,4 +1,4 @@
-// TMA-pipelined expert-parallel dispatch / combine for one NVSwitch node (sm_100a).
+// TMA-pipelined expert-parallel dispatch / combine for one NVSwitch node (sm_90a).
 //
 // Why a second implementation next to ep_kernels.cu: the register-path kernels keep one row per
 // warp in flight (LDG.128 -> registers -> STG.128), so the number of bytes in flight -- and with

@@ -1,4 +1,4 @@
-// AllReduce kernels for one NVSwitch node (2/4/8 ranks), all sm_100a, all operating
+// AllReduce kernels for one NVSwitch node (2/4/8 ranks), all sm_90a, all operating
 // directly on NVLink-mapped peer memory from the symmetric heap.
 //
 //   ar_oneshot<MC>     small messages: every rank pushes LL16 packets {data,flag,data,flag}

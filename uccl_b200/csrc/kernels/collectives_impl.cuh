@@ -311,8 +311,7 @@ __global__ void __launch_bounds__(512, 1) bcast_kernel(const __grid_constant__ D
   } else if constexpr (MODE == 3) {
     // ordinary output buffers + NVLS: the root stores every 16-byte word ONCE into the multicast address of the
     // staging area (the switch replicates it to all ranks), everybody copies its stage to the user buffer.  A pull from
-    // the root's stage would be bound by the root's egress (N - 1 copies of the message over one GPU's links:
-    // 111 GB/s on 8 GPUs vs 650 for NCCL).  Stage halves alternate, so one barrier per chunk suffices: the root
+    // the root's stage would be bound by the root's egress (N - 1 copies of the message over one GPU's links).  Stage halves alternate, so one barrier per chunk suffices: the root
     // rewrites half k & 1 only after the barrier of chunk k - 1, which every peer enters after copying chunk k - 2 out.
     const uint64_t half = (a.stage_bytes / 2) / 16 * 16;
     uint64_t k = 0;
@@ -535,8 +534,8 @@ namespace ub {
 //     sequence number in the receiver's heap; the receiver pulls the chunk over NVLink and acks.
 // Sequence counters are persistent and monotonic per (peer, sub-block): no reset, graph-replay safe.
 // (reference: lite's host-staged ncclSend/Recv, experimental/lite/nccl/nccl.cu:1145-1350,2033-2067;
-//  the first version of this kernel moved 512 KB slots with one 16-byte load in flight per thread and
-//  reached 9 GB/s in nccl-tests' alltoall_perf)
+//  the first version of this kernel moved 512 KB slots with one 16-byte load in flight per thread, far too
+//  few bytes in flight for NVLink)
 __device__ __forceinline__ void half_sync(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
 
 constexpr int kSrTmaStages = 8;      // receive half: bulk loads in flight (zero-copy pull and staged copy-out)

@@ -1,11 +1,11 @@
-// Device primitives for sm_100a communication kernels.
+// Device primitives for sm_90a communication kernels.
 //
 // What the reference provides here (behaviour, not code):
 //   * ep/include/ep_utils.cuh:259-395  L1-no-allocate loads/stores, sys-scope acquire/release
 //   * ep/include/ep_utils.cuh:447-585  TMA 1-D bulk copies + mbarrier helpers
 //   * experimental/lite/core/switch_channel_device.hpp:42-290  multimem.ld_reduce/st/red
 //   * experimental/lite/core/semaphore_device.hpp:66-145  device semaphores with spin caps
-// This file is the B200-native equivalent: every peer access is a plain global
+// This file is the Hopper-native equivalent: every peer access is a plain global
 // (or multimem) instruction on an NVLink-mapped VA from the symmetric heap.
 #pragma once
 #include <cuda_bf16.h>

@@ -2,7 +2,7 @@
 //
 // Role in the reference: collective/rdma/nccl_plugin.cc:85-633 (and the afxdp / efa twins) -- the object
 // NCCL loads through NCCL_NET_PLUGIN so that inter-node rings/trees run over UCCL's transport.  Inside a
-// B200 NVSwitch box NCCL never calls a net plugin; between boxes this one carries the traffic:
+// H100 NVSwitch box NCCL never calls a net plugin; between boxes this one carries the traffic:
 //
 //   NCCL_NET_PLUGIN=uccl_b200 LD_LIBRARY_PATH=$(python -c 'import uccl_b200;print(uccl_b200.lib_dir())') ...
 //

@@ -10,7 +10,7 @@
 //
 // Re-designed rather than ported: the packet I/O here is plain UDP sockets (P sockets = P source ports =
 // P ECMP paths) driven with sendmmsg/recvmmsg from ONE engine thread per NIC; the engine is the same
-// whether the bytes are host memory or a pinned staging buffer of the symmetric heap.  Inside a B200 box
+// whether the bytes are host memory or a pinned staging buffer of the symmetric heap.  Inside an H100 box
 // nothing here is used -- NVLink peers are load/store reachable -- this is the path *between* boxes, and
 // what the NCCL net plugin (csrc/net/nccl_net_plugin.cc) and `uccl_b200.net` are built on.
 //

@@ -3,10 +3,10 @@
 // Role in the reference: the UCCL-Tran packet formats -- `IMMData{FID,RID,CSN,HINT}` + the ACK/SACK
 // control header of the RDMA transport (collective/rdma/transport.h:122, transport_header.h) and the
 // `ucclh`/`ucclsackh` headers of the AF_XDP / DPDK / EFA transports.  Inside one NVSwitch node none of
-// this is needed (peers are load/store reachable); this is the scale-OUT path between B200 boxes.
+// this is needed (peers are load/store reachable); this is the scale-OUT path between H100 boxes.
 //
 // One datagram = PktHdr (+ type specific body) (+ payload).  All fields little endian (x86-64 / aarch64
-// hosts of B200 systems are both LE).  A flow is bidirectional; each direction numbers its reliable
+// hosts of H100 systems are both LE).  A flow is bidirectional; each direction numbers its reliable
 // packets independently.
 #pragma once
 #include <cstdint>

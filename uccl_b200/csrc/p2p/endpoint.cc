@@ -24,7 +24,7 @@ namespace ub {
 UB_PARAM(P2PCtas, "P2P_CTAS", 0)       // 0: by transfer size (8 / 32 / 64 CTAs)
 UB_PARAM(P2PChunkKB, "P2P_CHUNK_KB", 16)  // bytes per bulk copy; 4 pipelines x 3 stages of it per CTA
 UB_PARAM(P2PUseKernel, "P2P_USE_KERNEL", 1)
-// a handful of very large blocks is what the copy engines are best at (754 vs 700 GB/s at 512 MiB on 2 B200): up to 8
+// a handful of very large blocks is what the copy engines are best at: up to 8
 // blocks of at least this many MiB each go through cudaMemcpyAsync, everything else through the TMA copy kernel
 UB_PARAM(P2PMemcpyMinMB, "P2P_MEMCPY_MIN_MB", 32)
 // engine status line every N seconds at INFO level (reference: per-engine stats thread every 2 s unless

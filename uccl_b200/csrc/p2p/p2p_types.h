@@ -22,8 +22,7 @@ struct P2PCopyBatch {
   int n;
   uint32_t chunk_bytes;
   // n > kP2PMaxEntries: the descriptors live in a DEVICE table instead (filled through a pinned staging copy; a
-  // first version let the kernel read the pinned table itself and spent 1.8 ms on PCIe round trips for 1024
-  // blocks); one launch moves thousands of KV blocks.  `table_prefix` has n + 1 words
+  // first version let the kernel read the pinned table itself and paid a PCIe round trip per block); one launch moves thousands of KV blocks.  `table_prefix` has n + 1 words
   const P2PCopyEntry* table;
   const uint32_t* table_prefix;
   int any_tail;  // some entry is not a 16-byte multiple / aligned: the non-issuing lanes copy those bytes

@@ -5,8 +5,7 @@
 // peer's counter).
 //
 // Reference role: experimental/ukernel/src/device/persistent_kernel_ops.cu:180,262 -- here the
-// copy path is the same batched 16-byte ld/st engine the collectives use (saturates NVLink, see
-// profiles/), reductions accumulate 16/8-bit floats in fp32, and completion is published twice:
+// copy path is the same batched 16-byte ld/st engine the collectives use, reductions accumulate 16/8-bit floats in fp32, and completion is published twice:
 // to pinned host memory (CPU polling) and to device memory (cuStreamWaitValue64 by user streams).
 #include <stdio.h>
 

@@ -1,4 +1,4 @@
-"""DeepEP-compatible expert-parallel ``Buffer`` on top of the native sm_100a kernels.
+"""DeepEP-compatible expert-parallel ``Buffer`` on top of the native sm_90a kernels.
 
 API surface follows the reference's ``ep/bench/buffer.py`` (ctor :58-69, get_dispatch_layout
 :736, dispatch :837, combine :1190, low_latency_* :263-566, configs :680-733) so code written
@@ -190,7 +190,7 @@ class Buffer:
 
     @staticmethod
     def is_sm90_compiled() -> bool:
-        return True  # sm_100a build: every sm_90+ feature (fp8, TMA, clusters) is available
+        return True  # sm_90a build: every sm_90+ feature (fp8, TMA, clusters) is available
 
     @staticmethod
     def set_num_sms(new_num_sms: int) -> None:

@@ -1,4 +1,4 @@
-"""``uccl_b200.net`` -- the scale-OUT transport: multipath reliable datagrams between B200 boxes.
+"""``uccl_b200.net`` -- the scale-OUT transport: multipath reliable datagrams between H100 boxes.
 
 Inside one NVSwitch domain every peer is load/store reachable and nothing in this module is used.
 Between boxes the reference's core contribution applies (SURVEY N2 "UCCL-Tran", N6/N7 the AF_XDP / DPDK

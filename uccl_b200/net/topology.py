@@ -1,6 +1,6 @@
 """GPU <-> NIC matching for rail-aligned multi-node jobs.
 
-Each local rank should drive the NIC that hangs off the same PCIe switch as its GPU (on a B200 HGX board:
+Each local rank should drive the NIC that hangs off the same PCIe switch as its GPU (on an H100 HGX board:
 one ConnectX per GPU pair / GPU), so that staging traffic never crosses the CPU interconnect and every
 rail uses its own NIC.  The reference does this in its RDMA bring-up by comparing sysfs PCI paths
 (collective/rdma/util_rdma.*: GPU <-> NIC distance matrix).  Here it is a small pure function over the

@@ -18,6 +18,8 @@ from it are zero-copy for every collective (peer-mapped and multicast-bound).
 from __future__ import annotations
 
 import ctypes
+import os
+import warnings
 from typing import Iterable, List, Optional, Sequence
 
 import torch
@@ -148,6 +150,12 @@ class Communicator:
     def local_world(cls, world_size: Optional[int] = None, devices: Optional[Sequence[int]] = None,
                     heap_bytes: int = 1 << 30, stage_bytes: int = 64 << 20, host: Optional[bool] = None,
                     timeout_ms: int = -1, max_ctas: int = -1) -> List["Communicator"]:
+        """Communicators of every rank of a world inside this process, one per entry of `devices`.
+
+        A device listed more than once hosts *virtual ranks*: their kernels wait for each other inside one CUDA
+        context.  Under CUDA's lazy module loading the first launch of any kernel may synchronise that context, and
+        one issued while a virtual rank's kernel waits for its peer never returns.  Processes that use virtual
+        ranks must start with ``CUDA_MODULE_LOADING=EAGER`` (set before CUDA initialises); a warning says so."""
         C = _native.C()
         if host is None:
             host = not torch.cuda.is_available()
@@ -155,6 +163,9 @@ class Communicator:
             n = world_size or (1 if host else torch.cuda.device_count())
             devices = [-1] * n if host else [i % torch.cuda.device_count() for i in range(n)]
         if not host:
+            if len(set(devices)) < len(devices) and os.environ.get("CUDA_MODULE_LOADING", "").upper() != "EAGER":
+                warnings.warn("uccl_b200: virtual ranks (a device listed twice) can deadlock under lazy CUDA module "
+                              "loading; start the process with CUDA_MODULE_LOADING=EAGER", RuntimeWarning, stacklevel=2)
             torch.cuda.init()
         cs = C.Comm.create_local(list(devices), heap_bytes, stage_bytes, host, timeout_ms, max_ctas)
         return [cls(c) for c in cs]

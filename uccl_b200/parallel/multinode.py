@@ -1,4 +1,4 @@
-"""Collectives across several B200 boxes: NVLink inside a box, the datagram transport between boxes.
+"""Collectives across several H100 boxes: NVLink inside a box, the datagram transport between boxes.
 
 The reference scales out by plugging its transport under NCCL's rings.  With a full-bandwidth NVSwitch
 inside every box the better shape is hierarchical and *rail aligned*: local rank ``l`` of every node owns

@@ -1,6 +1,6 @@
 """SM partitions: a fixed set of a GPU's SMs (a CUDA green context) with streams bound to it.
 
-The communication kernels of this library run on an SM *budget* (expert parallelism: 24 of a B200's 148 SMs).  A grid
+The communication kernels of this library run on an SM *budget* (expert parallelism: 24 of an H100's 132 SMs).  A grid
 size only bounds how many CTAs a kernel brings; a partition also fixes where they run, so a GEMM that was launched first
 cannot keep the dispatch kernel waiting behind its waves, and the complementary partition keeps compute off the
 communication SMs.  Native side: ``csrc/common/sm_partition.{h,cc}``; the reference probes the same driver feature in

@@ -126,15 +126,15 @@ def tuning_from_sweep(sweep: dict) -> Dict[str, List[Tuple[int, str, int, float]
 
 
 def packaged_tuning_path(world_size: int) -> str:
-    """Measured table shipped with the package for an N x B200 NVSwitch box (uccl_b200/tuning/)."""
+    """Measured table shipped with the package for an N x H100 NVSwitch box (uccl_b200/tuning/)."""
     import os
 
-    return os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tuning", f"tuning_{world_size}xB200.json")
+    return os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tuning", f"tuning_{world_size}xH100.json")
 
 
 def load_tuning_from_env(comm) -> bool:
     """Install the table named by ``UCCL_B200_TUNE_FILE`` (written by :func:`save_tuning`); without the variable the
-    table measured on this box type for this world size (uccl_b200/tuning/tuning_<N>xB200.json) is used if it is
+    table measured on this box type for this world size (uccl_b200/tuning/tuning_<N>xH100.json) is used if it is
     shipped.  ``UCCL_B200_TUNE_FILE=none`` keeps the built-in thresholds of ``Comm::select_allreduce``."""
     import os
 
