@@ -116,6 +116,21 @@ PYBIND11_MODULE(_C, m) {
           },
           py::arg("inp"), py::arg("out"), py::arg("count"), py::arg("dtype"), py::arg("op"), py::arg("stream"),
           py::arg("algo") = 0, py::arg("scale") = 1.0f, py::arg("out_dtype") = -1, py::arg("max_ctas") = -1)
+      .def(
+          "allreduce_rmsnorm",
+          [](Comm& c, uintptr_t x, uintptr_t residual, uintptr_t residual_out, uintptr_t weight, uintptr_t out,
+             uintptr_t out_scales, size_t T, size_t H, int dtype, float eps, int quant, uintptr_t stream, int algo,
+             int max_ctas) {
+            ArOpts o;
+            o.algo = algo;
+            o.max_ctas = max_ctas;
+            py::gil_scoped_release rel;
+            c.allreduce_rmsnorm(P(x), P(residual), P(residual_out), P(weight), P(out),
+                                reinterpret_cast<float*>(out_scales), T, H, dtype, eps, quant, S(stream), o);
+          },
+          py::arg("x"), py::arg("residual"), py::arg("residual_out"), py::arg("weight"), py::arg("out"),
+          py::arg("out_scales"), py::arg("T"), py::arg("H"), py::arg("dtype"), py::arg("eps"), py::arg("quant"),
+          py::arg("stream"), py::arg("algo") = 0, py::arg("max_ctas") = -1)
       .def("allgather",
            [](Comm& c, uintptr_t in, uintptr_t out, size_t count, int dtype, uintptr_t stream) {
              py::gil_scoped_release rel;

@@ -466,6 +466,80 @@ void Comm::allreduce(const void* in, void* out, size_t count, int dtype, int op,
   UB_TRACE(SUB_COLL, "allreduce bytes=%zu algo=%s ctas=%d sym=%d", bytes, algo_name(algo), ctas, sym ? 1 : 0);
 }
 
+// ---------------------------------------------------------- allreduce + rmsnorm
+void Comm::allreduce_rmsnorm(void* x, const void* residual, void* residual_out, const void* weight, void* out,
+                             float* out_scales, size_t T, size_t H, int dtype, float eps, int quant,
+                             cudaStream_t stream, const ArOpts& opts) {
+  UB_CHECK(dtype == kBF16 || dtype == kF16, "allreduce_rmsnorm: dtype must be bf16 or fp16 (got %d)", dtype);
+  UB_CHECK(H >= 8 && H <= kRmsMaxH && H % 8 == 0, "allreduce_rmsnorm: hidden size %zu must be a multiple of 8 in [8, %u]",
+           H, kRmsMaxH);
+  UB_CHECK(quant == 0 || quant == 1, "allreduce_rmsnorm: bad quant %d", quant);
+  UB_CHECK(!quant || H % 128 == 0, "allreduce_rmsnorm: fp8 output needs hidden size %% 128 == 0 (got %zu)", H);
+  UB_CHECK(T <= UINT32_MAX, "allreduce_rmsnorm: too many rows (%zu)", T);
+  if (T == 0) return;
+  check_buf(x, "x");
+  check_buf(residual, "residual");
+  check_buf(residual_out, "residual_out");
+  check_buf(weight, "weight");
+  check_buf(out, "out");
+  if (quant) check_buf(out_scales, "out_scales");
+  float* scales = quant ? out_scales : nullptr;
+  const int n = nranks();
+  const size_t count = T * H, bytes = count * dtype_size(dtype);
+  if (is_host()) {
+    host_allreduce(x, x, count, dtype, kSum, 1.0f, dtype);
+    host_add_rmsnorm(x, residual, residual_out, weight, out, scales, T, H, dtype, eps);
+    return;
+  }
+  DeviceGuard g(device());
+  UB_CHECK(aligned16(x) && aligned16(residual) && aligned16(residual_out) && aligned16(weight) && aligned16(out),
+           "allreduce_rmsnorm: x, residual, residual_out, weight and out must be 16-byte aligned");
+  RmsNormArgs r;
+  r.x = x;
+  r.residual = residual;
+  r.residual_out = residual_out;
+  r.weight = weight;
+  r.out = out;
+  r.out_scales = scales;
+  r.T = (uint32_t)T;
+  r.H = (uint32_t)H;
+  r.eps = eps;
+
+  // the fused kernel takes exactly the sizes for which the plain all-reduce would run one-shot
+  int algo = opts.algo, ctas = 0;
+  if (algo == ALGO_AUTO && n > 1) algo = select_allreduce(bytes, in_heap(x, bytes), dtype, kSum, &ctas);
+  if (algo == ALGO_ONESHOT_LL || algo == ALGO_ONESHOT_MC) {
+    UB_CHECK(algo == ALGO_ONESHOT_LL || has_multicast(), "allreduce_rmsnorm: algo %s needs NVLS multicast",
+             algo_name(algo));
+    UB_CHECK(bytes <= kLLMaxData, "allreduce_rmsnorm: one-shot limited to %lu bytes", (unsigned long)kLLMaxData);
+    if (ctas <= 0) ctas = ctas_for(bytes, std::min(max_ctas_, 64), 8192);
+    if (opts.max_ctas > 0) ctas = std::min(ctas, opts.max_ctas);
+    ctas = (int)std::min<size_t>(ctas, T);  // a block owns whole rows
+    CollArgs a = base_args();
+    a.in = x;
+    a.out = x;
+    a.bytes = bytes;
+    a.count = count;
+    cudaError_t e = launch_allreduce_rmsnorm(algo, dtype, quant != 0, dev_, a, r, ctas, stream);
+    UB_CHECK(e == cudaSuccess, "allreduce_rmsnorm launch failed (rank %d algo=%s ctas=%d): %s", rank(),
+             algo_name(algo), ctas, cudaGetErrorString(e));
+    ++launches_;
+    UB_TRACE(SUB_COLL, "allreduce_rmsnorm fused T=%zu H=%zu algo=%s ctas=%d", T, H, algo_name(algo), ctas);
+    return;
+  }
+  if (n > 1) {
+    ArOpts o;
+    o.algo = opts.algo;  // AUTO re-selects the same algorithm
+    o.max_ctas = opts.max_ctas;
+    allreduce(x, x, count, dtype, kSum, stream, o);
+  }
+  const int grid = (int)std::min<size_t>(T, 1024);
+  cudaError_t e = launch_allreduce_rmsnorm(0, dtype, quant != 0, dev_, base_args(), r, grid, stream);
+  UB_CHECK(e == cudaSuccess, "add_rmsnorm launch failed (rank %d): %s", rank(), cudaGetErrorString(e));
+  ++launches_;
+  UB_TRACE(SUB_COLL, "allreduce_rmsnorm unfused T=%zu H=%zu algo=%s", T, H, algo_name(algo));
+}
+
 // ------------------------------------------------------------------ allgather
 void Comm::allgather(const void* in, void* out, size_t count_per_rank, int dtype, cudaStream_t stream) {
   UB_CHECK(dtype >= 0 && dtype < kNumDTypes, "allgather: bad dtype %d", dtype);

@@ -92,6 +92,13 @@ class Comm {
   void alltoallv(const void* in, const size_t* send_counts, const size_t* send_displs, void* out,
                  const size_t* recv_counts, const size_t* recv_displs, int dtype, cudaStream_t stream);
   void barrier(cudaStream_t stream);
+  // In-place sum all-reduce of x [T, H], then residual_out = x + residual and out = rmsnorm(residual_out) * weight
+  // (quant = 1: out is e4m3 with fp32 inverse scales per 128 channels in out_scales [T, H / 128]).  bf16 / fp16,
+  // H % 8 == 0, H <= kRmsMaxH.  The fused one-shot kernel runs where AUTO picks a one-shot all-reduce (or
+  // opts.algo forces one); otherwise the selected all-reduce runs, followed by the local epilogue kernel.
+  void allreduce_rmsnorm(void* x, const void* residual, void* residual_out, const void* weight, void* out,
+                         float* out_scales, size_t T, size_t H, int dtype, float eps, int quant, cudaStream_t stream,
+                         const ArOpts& opts = ArOpts());
   // grouped point-to-point (ncclGroupStart .. ncclSend/ncclRecv .. ncclGroupEnd)
   struct P2pOp {
     bool is_send;
@@ -165,6 +172,9 @@ const char* algo_name(int algo);
 
 // CPU reference reduction used by the host backends: dst[i] = op_r srcs[r][i], then * scale (floats)
 void host_reduce_n(void* dst, const void* const* srcs, int n, size_t count, int dtype, int op, float scale);
+// CPU epilogue of allreduce_rmsnorm on an already reduced x (bf16 / fp16, fp32 arithmetic; e4m3 when out_scales)
+void host_add_rmsnorm(const void* x, const void* residual, void* residual_out, const void* weight, void* out,
+                      float* out_scales, size_t T, size_t H, int dtype, float eps);
 
 // torch.cuda.MemPool backend (mem_pool.cc): which communicator serves `uccl_b200_pool_malloc`
 void pool_install(std::shared_ptr<Comm> c);            // default for c->device()

@@ -7,9 +7,11 @@
 // (experimental/ukernel/src/ccl/test/common/backend_test_utils.h:211).
 #include <sched.h>
 
+#include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <cstring>
+#include <vector>
 
 #include "../common/log.h"
 #include "comm.h"
@@ -206,6 +208,62 @@ bool reduce2_fast(void* dst, const void* a, const void* b, size_t n, int dtype, 
 void host_reduce_n(void* dst, const void* const* srcs, int n, size_t count, int dtype, int op, float scale) {
   if (n == 2 && scale == 1.0f && reduce2_fast(dst, srcs[0], srcs[1], count, dtype, op)) return;
   reduce_n(dst, srcs, n, count, dtype, op, scale);
+}
+
+namespace {
+// fp32 -> e4m3 (finite-only format, max 448): round to nearest even, saturating like the device conversion
+uint8_t f32_to_e4m3(float f) {
+  uint32_t u;
+  memcpy(&u, &f, 4);
+  const uint8_t sign = (uint8_t)((u >> 24) & 0x80u);
+  const float a = std::fabs(f);
+  if (std::isnan(f)) return sign | 0x7f;
+  if (a >= 448.0f) return sign | 0x7e;
+  if (a < 0.015625f) return sign | (uint8_t)std::nearbyint(a * 512.0f);  // subnormals: multiples of 2^-9
+  int e = (int)((u >> 23) & 0xff) - 127;                                  // -6 .. 8
+  int q = (int)std::nearbyint(std::ldexp(a, 3 - e));                       // 8 .. 16
+  if (q == 16) {
+    q = 8;
+    ++e;
+  }
+  return sign | (uint8_t)(((e + 7) << 3) | (q - 8));
+}
+}  // namespace
+
+void host_add_rmsnorm(const void* x, const void* residual, void* residual_out, const void* weight, void* out,
+                      float* out_scales, size_t T, size_t H, int dtype, float eps) {
+  const bool bf = dtype == kBF16;
+  auto ld = [bf](const void* p, size_t i) {
+    const uint16_t h = static_cast<const uint16_t*>(p)[i];
+    return bf ? bf16_to_f32(h) : f16_to_f32(h);
+  };
+  auto rnd = [bf](float v) { return bf ? f32_to_bf16(v) : f32_to_f16(v); };
+  std::vector<float> r(H), y(H);
+  for (size_t t = 0; t < T; ++t) {
+    const size_t o = t * H;
+    float ss = 0.f;
+    for (size_t i = 0; i < H; ++i) {  // read the whole row first: residual_out may alias residual
+      const uint16_t h = rnd(ld(x, o + i) + ld(residual, o + i));
+      r[i] = bf ? bf16_to_f32(h) : f16_to_f32(h);
+      ss += r[i] * r[i];
+    }
+    for (size_t i = 0; i < H; ++i) static_cast<uint16_t*>(residual_out)[o + i] = rnd(r[i]);
+    const float inv = 1.0f / std::sqrt(ss / (float)H + eps);
+    for (size_t i = 0; i < H; ++i) {
+      const uint16_t h = rnd(r[i] * inv * ld(weight, i));
+      if (!out_scales) static_cast<uint16_t*>(out)[o + i] = h;
+      y[i] = bf ? bf16_to_f32(h) : f16_to_f32(h);
+    }
+    if (!out_scales) continue;
+    for (size_t g = 0; g < H / 128; ++g) {
+      float amax = 0.f;
+      for (size_t i = 0; i < 128; ++i) amax = std::max(amax, std::fabs(y[g * 128 + i]));
+      amax = std::max(amax, 1e-4f);
+      const float scale = (1.0f / amax) * 448.0f;  // rounded like per_token_cast_to_fp8 (see fp8_quant.cuh)
+      out_scales[t * (H / 128) + g] = amax / 448.0f;
+      for (size_t i = 0; i < 128; ++i) static_cast<uint8_t*>(out)[o + g * 128 + i] = f32_to_e4m3(y[g * 128 + i] * scale);
+    }
+  }
 }
 
 void Comm::host_barrier() {

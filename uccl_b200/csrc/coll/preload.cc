@@ -51,6 +51,13 @@ cudaError_t preload_all_kernels() {
     ok(launch_allreduce_f(algo, kBF16, kSum, kF32, c, a, 1, 512, 0));
     ok(launch_allreduce_f(algo, kF16, kSum, kF32, c, a, 1, 512, 0));
   }
+  {
+    RmsNormArgs r;
+    memset(&r, 0, sizeof(r));
+    for (int algo : {0, 1, 2})
+      for (int dt : {(int)kBF16, (int)kF16})
+        for (bool fp8 : {false, true}) ok(launch_allreduce_rmsnorm(algo, dt, fp8, c, a, r, 1, 0));
+  }
   for (int m = 0; m < 5; ++m) ok(launch_allgather(m, c, a, 1, 512, 0));
   for (int m = 0; m < 4; ++m) ok(launch_broadcast(m, c, a, 1, 512, 0));
   for (int m = 0; m < 3; ++m) ok(launch_alltoall(m, c, a, 1, 512, 0));

@@ -1,7 +1,8 @@
 // Device code shared by the register-path (ep_kernels.cu) and the TMA-pipelined (ep_tma_kernels.cu)
-// expert-parallel kernels: bf16 <-> fp32 / e4m3 helpers, the per-128-channel quantiser and the
-// count-exchange prologue of a non-cached dispatch.
+// expert-parallel kernels: bf16 -> fp32 helper, the per-128-channel quantiser (kernels/fp8_quant.cuh)
+// and the count-exchange prologue of a non-cached dispatch.
 #pragma once
+#include "../kernels/fp8_quant.cuh"
 #include "../kernels/prims.cuh"
 #include "ep_types.h"
 
@@ -14,29 +15,6 @@ __device__ __forceinline__ void bf16x8_to_float(const uint4& v, float (&f)[8]) {
     float2 p = __bfloat1622float2(h[i]);
     f[2 * i] = p.x;
     f[2 * i + 1] = p.y;
-  }
-}
-
-__device__ __forceinline__ uint32_t pack4_e4m3(float a, float b, float c, float d) {
-  __nv_fp8x2_storage_t lo = __nv_cvt_float2_to_fp8x2(make_float2(a, b), __NV_SATFINITE, __NV_E4M3);
-  __nv_fp8x2_storage_t hi = __nv_cvt_float2_to_fp8x2(make_float2(c, d), __NV_SATFINITE, __NV_E4M3);
-  return (uint32_t)lo | ((uint32_t)hi << 16);
-}
-
-
-// scale / inverse scale of one 128-channel group from its amax (bit-identical to the torch reference
-// `amax.clamp(1e-4) / 448`; round_scale: power-of-two inverse scale, UE8M0 compatible)
-__device__ __forceinline__ void fp8_group_scale(float amax, int round_scale, float& scale, float& scale_inv) {
-  amax = fmaxf(amax, 1e-4f);
-  if (round_scale) {
-    const float raw = amax * (1.0f / 448.0f);
-    int ex = ((__float_as_int(raw) >> 23) & 0xff) - 127;
-    if ((__float_as_int(raw) & 0x7fffff) != 0) ex += 1;
-    scale_inv = __int_as_float((ex + 127) << 23);
-    scale = __int_as_float((127 - ex) << 23);
-  } else {
-    scale = 448.0f / amax;
-    scale_inv = __fdiv_rn(amax, 448.0f);
   }
 }
 

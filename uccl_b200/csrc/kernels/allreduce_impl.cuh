@@ -27,79 +27,75 @@
 namespace ub {
 
 // ------------------------------------------------------------------ one-shot LL
-template <typename T, int OP, bool MC>
-__global__ void __launch_bounds__(512) ar_oneshot(const __grid_constant__ DevComm c,
-                                                  const __grid_constant__ CollArgs a) {
-  uint32_t* misc = reinterpret_cast<uint32_t*>(c.heap[c.rank] + a.misc_off);
+// The LL protocol below is shared by ar_oneshot and the fused all-reduce + RMSNorm kernel
+// (allreduce_rmsnorm.cu).  Both use the same epoch words and packet slots, so plain and fused one-shot
+// launches may be interleaved on a stream or inside one CUDA graph.
+
+// Flag of this launch: the epoch left by the previous one-shot launch + 1.  Every thread must call it.
+__device__ __forceinline__ uint32_t ll_begin(const uint32_t* misc) {
   __shared__ uint32_t s_flag;
   if (threadIdx.x == 0) s_flag = ld_volatile(misc + kLLEpoch) + 1;
   __syncthreads();
-  const uint32_t flag = s_flag;
-  const uint64_t parity_off = a.ll_off + (uint64_t)(flag & 1u) * (kMaxRanks * kLLSlotBytes);
-  const uint64_t nunits = (a.bytes + 15) / 16;
-  const uint64_t gtid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const uint64_t gstride = (uint64_t)gridDim.x * blockDim.x;
-  const int n = c.nranks, rank = c.rank;
+  return s_flag;
+}
 
-  // phase 1: publish my data as packets into every peer's slot[rank] (4 loads in flight per thread)
-  {
-    constexpr int B = 4;
-    for (uint64_t u0 = gtid; u0 < nunits; u0 += gstride * B) {
-      uint4 d[B];
+__device__ __forceinline__ uint64_t ll_parity_off(const CollArgs& a, uint32_t flag) {
+  return a.ll_off + (uint64_t)(flag & 1u) * (kMaxRanks * kLLSlotBytes);
+}
+
+// Publish 16-byte units first, first + stride, ... (< end) of a.in as packets {data,flag,data,flag} into every
+// peer's slot[rank] (4 loads in flight per thread).
+template <bool MC>
+__device__ __forceinline__ void ll_publish(const DevComm& c, const CollArgs& a, uint32_t flag, uint64_t parity_off,
+                                           uint64_t first, uint64_t end, uint64_t stride) {
+  constexpr int B = 4;
+  const int n = c.nranks, rank = c.rank;
+  for (uint64_t u0 = first; u0 < end; u0 += stride * B) {
+    uint4 d[B];
 #pragma unroll
-      for (int j = 0; j < B; ++j) {
-        const uint64_t u = u0 + (uint64_t)j * gstride;
-        if (u < nunits) d[j] = load16_partial(a.in, u * 16, a.bytes);
-      }
-#pragma unroll
-      for (int j = 0; j < B; ++j) {
-        const uint64_t u = u0 + (uint64_t)j * gstride;
-        if (u >= nunits) continue;
-        uint4 p0 = make_uint4(d[j].x, flag, d[j].y, flag);
-        uint4 p1 = make_uint4(d[j].z, flag, d[j].w, flag);
-        const uint64_t off = parity_off + (uint64_t)rank * kLLSlotBytes + u * 32;
-        if constexpr (MC) {
-          multimem_st_v4(c.mc + off, p0);
-          multimem_st_v4(c.mc + off + 16, p1);
-        } else {
-          for (int k = 1; k < n; ++k) {
-            int p = rank + k;
-            if (p >= n) p -= n;
-            st_v4(c.heap[p] + off, p0);
-            st_v4(c.heap[p] + off + 16, p1);
-          }
-        }
-      }
+    for (int j = 0; j < B; ++j) {
+      const uint64_t u = u0 + (uint64_t)j * stride;
+      if (u < end) d[j] = load16_partial(a.in, u * 16, a.bytes);
     }
-  }
-  // phase 2: wait for the peers' packets in my own scratch, reduce in rank order
-  // (identical order on every rank => bitwise identical results everywhere)
-  char* my_ll = c.heap[rank] + parity_off;
-  for (uint64_t u = gtid; u < nunits; u += gstride) {
-    Vec16<T, OP> acc;
-    for (int s = 0; s < n; ++s) {
-      uint4 d;
-      if (s == rank) {
-        d = load16_partial(a.in, u * 16, a.bytes);
+#pragma unroll
+    for (int j = 0; j < B; ++j) {
+      const uint64_t u = u0 + (uint64_t)j * stride;
+      if (u >= end) continue;
+      uint4 p0 = make_uint4(d[j].x, flag, d[j].y, flag);
+      uint4 p1 = make_uint4(d[j].z, flag, d[j].w, flag);
+      const uint64_t off = parity_off + (uint64_t)rank * kLLSlotBytes + u * 32;
+      if constexpr (MC) {
+        multimem_st_v4(c.mc + off, p0);
+        multimem_st_v4(c.mc + off + 16, p1);
       } else {
-        const char* slot = my_ll + (uint64_t)s * kLLSlotBytes + u * 32;
-        uint4 p0, p1;
-        SpinGuard g(c.timeout_ns);
-        while (true) {
-          p0 = ld_volatile_v4(slot);
-          p1 = ld_volatile_v4(slot + 16);
-          if (p0.y == flag && p0.w == flag && p1.y == flag && p1.w == flag) break;
-          if (g.expired()) comm_abort(c, 10, s, (int)flag);
+        for (int k = 1; k < n; ++k) {
+          int p = rank + k;
+          if (p >= n) p -= n;
+          st_v4(c.heap[p] + off, p0);
+          st_v4(c.heap[p] + off + 16, p1);
         }
-        d = make_uint4(p0.x, p0.z, p1.x, p1.z);
       }
-      if (s == 0) acc.init(d);
-      else acc.accum(d);
     }
-    acc.epilogue(a.ep);
-    store16_partial(a.out, u * 16, a.bytes, acc.pack_same());
   }
-  // last block to finish bumps the epoch (graph-replay safe: no host-side counter)
+}
+
+// Wait for rank s's packet of unit u in my own scratch (my_ll = my heap + parity_off); returns its 16 data bytes.
+__device__ __forceinline__ uint4 ll_recv(const DevComm& c, const char* my_ll, int s, uint64_t u, uint32_t flag) {
+  const char* slot = my_ll + (uint64_t)s * kLLSlotBytes + u * 32;
+  uint4 p0, p1;
+  SpinGuard g(c.timeout_ns);
+  while (true) {
+    p0 = ld_volatile_v4(slot);
+    p1 = ld_volatile_v4(slot + 16);
+    if (p0.y == flag && p0.w == flag && p1.y == flag && p1.w == flag) break;
+    if (g.expired()) comm_abort(c, 10, s, (int)flag);
+  }
+  return make_uint4(p0.x, p0.z, p1.x, p1.z);
+}
+
+// The last block of the launch to finish bumps the epoch (graph-replay safe: no host-side counter).
+// Every thread must call it.
+__device__ __forceinline__ void ll_end(uint32_t* misc, uint32_t flag) {
   __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence();
@@ -110,6 +106,35 @@ __global__ void __launch_bounds__(512) ar_oneshot(const __grid_constant__ DevCom
       __threadfence();
     }
   }
+}
+
+template <typename T, int OP, bool MC>
+__global__ void __launch_bounds__(512) ar_oneshot(const __grid_constant__ DevComm c,
+                                                  const __grid_constant__ CollArgs a) {
+  uint32_t* misc = reinterpret_cast<uint32_t*>(c.heap[c.rank] + a.misc_off);
+  const uint32_t flag = ll_begin(misc);
+  const uint64_t parity_off = ll_parity_off(a, flag);
+  const uint64_t nunits = (a.bytes + 15) / 16;
+  const uint64_t gtid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const uint64_t gstride = (uint64_t)gridDim.x * blockDim.x;
+  const int n = c.nranks, rank = c.rank;
+
+  // phase 1: publish my data as packets into every peer's slot[rank]
+  ll_publish<MC>(c, a, flag, parity_off, gtid, nunits, gstride);
+  // phase 2: wait for the peers' packets in my own scratch, reduce in rank order
+  // (identical order on every rank => bitwise identical results everywhere)
+  const char* my_ll = c.heap[rank] + parity_off;
+  for (uint64_t u = gtid; u < nunits; u += gstride) {
+    Vec16<T, OP> acc;
+    for (int s = 0; s < n; ++s) {
+      const uint4 d = s == rank ? load16_partial(a.in, u * 16, a.bytes) : ll_recv(c, my_ll, s, u, flag);
+      if (s == 0) acc.init(d);
+      else acc.accum(d);
+    }
+    acc.epilogue(a.ep);
+    store16_partial(a.out, u * 16, a.bytes, acc.pack_same());
+  }
+  ll_end(misc, flag);
 }
 
 // ------------------------------------------------------------ two-shot zero-copy

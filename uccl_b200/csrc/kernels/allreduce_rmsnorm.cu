@@ -1,0 +1,193 @@
+// All-reduce (sum) fused with the residual add and RMSNorm that follow every row-parallel GEMM of a
+// tensor-parallel transformer, optionally quantised to e4m3 for an fp8 GEMM or an EP dispatch:
+//
+//   x            = sum_r x_r                          (fp32 in rank order, rounded once; in place)
+//   residual_out = T(x + residual)
+//   out          = T(residual_out * rsqrt(mean(residual_out^2) + eps) * weight)   [-> e4m3 + scales]
+//
+//   ar_oneshot_rmsnorm<T, MC, FP8>  the one-shot LL all-reduce (allreduce_impl.cuh) with row-owned phases: block b
+//                                   publishes and reduces rows b, b + grid, ... and runs the row epilogue on the
+//                                   reduced row while it is still in registers.  No barrier, no extra HBM pass.
+//   add_rmsnorm_kernel<T, FP8>      the same row epilogue on an already reduced x (the unfused path behind the
+//                                   two-shot / staged / NVLS all-reduce, and one-rank communicators).
+// Both run the identical epilogue with the identical thread -> element mapping, so their results are bitwise equal.
+#include "allreduce_impl.cuh"
+#include "fp8_quant.cuh"
+
+namespace ub {
+
+template <typename T>
+__device__ __forceinline__ float round_to(float v) {
+  return to_acc<float, T>(from_acc<T, float>(v));
+}
+
+// Row epilogue.  v[k] holds the reduced values (already rounded to T) of unit k * kRmsThreads + threadIdx.x of
+// the row.  The whole residual row is loaded before anything is stored, and every thread only stores the units
+// it loaded, so residual_out may alias residual.  All kRmsThreads threads of the block must call it.
+template <typename T, bool FP8>
+__device__ __forceinline__ void rmsnorm_row(float (&v)[kRmsUnits][8], uint64_t row, const RmsNormArgs& r,
+                                            float* s_warp) {
+  const int tid = threadIdx.x;
+  const uint32_t upr = r.H / 8;  // 16-byte units per row
+  const uint64_t base = row * upr;
+  uint4 res[kRmsUnits];
+#pragma unroll
+  for (int k = 0; k < kRmsUnits; ++k) {
+    const uint32_t u = k * kRmsThreads + tid;
+    if (u < upr) res[k] = ld_v4(static_cast<const char*>(r.residual) + (base + u) * 16);
+  }
+  // residual add, rounded to T; sum of squares of the rounded values in a fixed order
+  float ss = 0.f;
+#pragma unroll
+  for (int k = 0; k < kRmsUnits; ++k) {
+    const uint32_t u = k * kRmsThreads + tid;
+    if (u < upr) {
+      Vec16<T, kSum> rv;
+      rv.init(res[k]);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        rv.a[i] = round_to<T>(v[k][i] + rv.a[i]);
+        v[k][i] = rv.a[i];
+        ss = __fmaf_rn(rv.a[i], rv.a[i], ss);
+      }
+      st_v4(static_cast<char*>(r.residual_out) + (base + u) * 16, rv.pack_same());
+    }
+  }
+  // block sum: butterfly inside each warp, then the warp partials in warp order
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+  if ((tid & 31) == 0) s_warp[tid >> 5] = ss;
+  __syncthreads();
+  float tot = 0.f;
+#pragma unroll
+  for (int w = 0; w < kRmsThreads / 32; ++w) tot += s_warp[w];
+  __syncthreads();  // s_warp is reused by the next row
+  const float inv = rsqrtf(__fdiv_rn(tot, (float)r.H) + r.eps);
+
+#pragma unroll
+  for (int k = 0; k < kRmsUnits; ++k) {
+    if (k * kRmsThreads >= (int)upr) break;  // block-uniform: the fp8 path shuffles below
+    const uint32_t u = k * kRmsThreads + tid;
+    const bool valid = u < upr;
+    Vec16<T, kSum> y;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) y.a[i] = 0.f;
+    if (valid) {
+      Vec16<T, kSum> w;
+      w.init(ld_nc_v4(static_cast<const char*>(r.weight) + (uint64_t)u * 16));
+#pragma unroll
+      for (int i = 0; i < 8; ++i) y.a[i] = round_to<T>(__fmul_rn(__fmul_rn(v[k][i], inv), w.a[i]));
+    }
+    if constexpr (!FP8) {
+      if (valid) st_v4(static_cast<char*>(r.out) + (base + u) * 16, y.pack_same());
+    } else {
+      // one 128-channel group = 16 consecutive units = 16 consecutive lanes (kRmsThreads and upr are multiples of 16)
+      float amax = 0.f;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) amax = fmaxf(amax, fabsf(y.a[i]));
+#pragma unroll
+      for (int o = 1; o < 16; o <<= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+      float scale, scale_inv;
+      fp8_group_scale_torch(amax, scale, scale_inv);
+      uint2 q;
+      q.x = pack4_e4m3(y.a[0] * scale, y.a[1] * scale, y.a[2] * scale, y.a[3] * scale);
+      q.y = pack4_e4m3(y.a[4] * scale, y.a[5] * scale, y.a[6] * scale, y.a[7] * scale);
+      if (valid) {
+        st_v2(static_cast<char*>(r.out) + (base + u) * 8, q);
+        if ((tid & 15) == 0) r.out_scales[row * (r.H / 128) + u / 16] = scale_inv;
+      }
+    }
+  }
+}
+
+// Fused path: the one-shot LL all-reduce of allreduce_impl.cuh (same epoch words, packet slots and spin sites)
+// with row-owned phases.  A block publishes exactly the rows it later reduces, with the same thread -> unit
+// mapping, so storing the sum over x in place never races with another block still publishing x.
+// The grid must not exceed the one-shot's: with virtual ranks every rank's blocks have to be resident at once.
+template <typename T, bool MC, bool FP8>
+__global__ void __launch_bounds__(kRmsThreads) ar_oneshot_rmsnorm(const __grid_constant__ DevComm c,
+                                                                  const __grid_constant__ CollArgs a,
+                                                                  const __grid_constant__ RmsNormArgs r) {
+  __shared__ float s_warp[kRmsThreads / 32];
+  uint32_t* misc = reinterpret_cast<uint32_t*>(c.heap[c.rank] + a.misc_off);
+  const uint32_t flag = ll_begin(misc);
+  const uint64_t parity_off = ll_parity_off(a, flag);
+  const uint32_t upr = r.H / 8;
+  const int n = c.nranks, rank = c.rank, tid = threadIdx.x;
+
+  for (uint64_t row = blockIdx.x; row < r.T; row += gridDim.x)
+    ll_publish<MC>(c, a, flag, parity_off, row * upr + tid, (row + 1) * upr, kRmsThreads);
+
+  const char* my_ll = c.heap[rank] + parity_off;
+  char* x = static_cast<char*>(r.x);
+  for (uint64_t row = blockIdx.x; row < r.T; row += gridDim.x) {
+    float v[kRmsUnits][8];
+#pragma unroll
+    for (int k = 0; k < kRmsUnits; ++k) {
+      const uint32_t ur = k * kRmsThreads + tid;
+      if (ur >= upr) continue;
+      const uint64_t u = row * upr + ur;
+      Vec16<T, kSum> acc;
+      for (int s = 0; s < n; ++s) {
+        const uint4 d = s == rank ? ld_v4(x + u * 16) : ll_recv(c, my_ll, s, u, flag);
+        if (s == 0) acc.init(d);
+        else acc.accum(d);
+      }
+      const uint4 sum = acc.pack_same();
+      st_v4(x + u * 16, sum);
+      Vec16<T, kSum> rounded;
+      rounded.init(sum);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) v[k][i] = rounded.a[i];
+    }
+    rmsnorm_row<T, FP8>(v, row, r, s_warp);
+  }
+  ll_end(misc, flag);
+}
+
+template <typename T, bool FP8>
+__global__ void __launch_bounds__(kRmsThreads) add_rmsnorm_kernel(const __grid_constant__ RmsNormArgs r) {
+  __shared__ float s_warp[kRmsThreads / 32];
+  const uint32_t upr = r.H / 8;
+  const char* x = static_cast<const char*>(r.x);
+  for (uint64_t row = blockIdx.x; row < r.T; row += gridDim.x) {
+    float v[kRmsUnits][8];
+#pragma unroll
+    for (int k = 0; k < kRmsUnits; ++k) {
+      const uint32_t ur = k * kRmsThreads + threadIdx.x;
+      if (ur >= upr) continue;
+      Vec16<T, kSum> xv;
+      xv.init(ld_v4(x + (row * upr + ur) * 16));
+#pragma unroll
+      for (int i = 0; i < 8; ++i) v[k][i] = xv.a[i];
+    }
+    rmsnorm_row<T, FP8>(v, row, r, s_warp);
+  }
+}
+
+template <typename T, bool FP8>
+static cudaError_t launch_rms_typed(int algo, const DevComm& c, const CollArgs& a, const RmsNormArgs& r, int grid,
+                                    cudaStream_t st) {
+  switch (algo) {
+    case 0: UB_LAUNCH((add_rmsnorm_kernel<T, FP8>), grid, kRmsThreads, 0, st, r); break;
+    case AR_ONESHOT_LL: UB_LAUNCH((ar_oneshot_rmsnorm<T, false, FP8>), grid, kRmsThreads, 0, st, c, a, r); break;
+    case AR_ONESHOT_MC: UB_LAUNCH((ar_oneshot_rmsnorm<T, true, FP8>), grid, kRmsThreads, 0, st, c, a, r); break;
+    default: return cudaErrorInvalidValue;
+  }
+  return cudaGetLastError();
+}
+
+cudaError_t launch_allreduce_rmsnorm(int algo, int dtype, bool fp8, const DevComm& c, const CollArgs& a,
+                                     const RmsNormArgs& r, int grid, cudaStream_t st) {
+  switch (dtype) {
+    case kBF16:
+      return fp8 ? launch_rms_typed<__nv_bfloat16, true>(algo, c, a, r, grid, st)
+                 : launch_rms_typed<__nv_bfloat16, false>(algo, c, a, r, grid, st);
+    case kF16:
+      return fp8 ? launch_rms_typed<__half, true>(algo, c, a, r, grid, st)
+                 : launch_rms_typed<__half, false>(algo, c, a, r, grid, st);
+    default: return cudaErrorInvalidValue;
+  }
+}
+
+}  // namespace ub

@@ -31,6 +31,11 @@ cudaError_t launch_allreduce_i(int algo, int dtype, int op, const DevComm& c, co
                                int block, cudaStream_t st);
 cudaError_t launch_allreduce_x(int algo, int dtype, int op, const DevComm& c, const CollArgs& a, int grid,
                                int block, cudaStream_t st);
+// all-reduce (sum) + residual add + RMSNorm [+ e4m3 cast] (allreduce_rmsnorm.cu): algo AR_ONESHOT_LL / AR_ONESHOT_MC
+// launch the fused one-shot kernel (a = one-shot arguments with in = out = r.x), algo 0 the local epilogue on an
+// already reduced r.x.  dtype kBF16 / kF16; fp8 = e4m3 output with per-128-channel scales.
+cudaError_t launch_allreduce_rmsnorm(int algo, int dtype, bool fp8, const DevComm& c, const CollArgs& a,
+                                     const RmsNormArgs& r, int grid, cudaStream_t st);
 // allgather modes: 0 push P2P, 1 push multicast, 2 pull/staged, 3 LL packets, 4 LL packets via multicast
 cudaError_t launch_allgather(int mode, const DevComm& c, const CollArgs& a, int grid, int block, cudaStream_t st);
 cudaError_t launch_broadcast(int mode, const DevComm& c, const CollArgs& a, int grid, int block, cudaStream_t st);

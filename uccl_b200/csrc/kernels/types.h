@@ -136,6 +136,22 @@ struct CollArgs {
   uint64_t misc_off, ll_off, stage_in_off, stage_out_off, stage_bytes;
 };
 
+// Fused all-reduce + residual add + RMSNorm (allreduce_rmsnorm.cu).  One CTA of kRmsThreads threads holds a
+// row in registers, at most kRmsUnits 16-byte units per thread, hence H <= kRmsMaxH for 16-bit dtypes.
+constexpr int kRmsThreads = 512;
+constexpr int kRmsUnits = 4;
+constexpr uint32_t kRmsMaxH = (uint32_t)kRmsThreads * kRmsUnits * 8;
+struct RmsNormArgs {
+  void* x;                 // [T, H]: the reduced sum (stored by the fused kernel, read by the local one)
+  const void* residual;    // [T, H]
+  void* residual_out;      // [T, H] = x + residual; may equal residual
+  const void* weight;      // [H]
+  void* out;               // [T, H] of the input dtype, or e4m3 when out_scales != nullptr
+  float* out_scales;       // [T, H / 128] inverse scales of the e4m3 output (nullptr: no quantisation)
+  uint32_t T, H;
+  float eps;
+};
+
 // Split [0, total) into `parts` nearly equal contiguous ranges whose boundaries are
 // multiples of `gran` (except the final end).
 UB_HD inline void split_range(uint64_t total, int parts, int idx, uint64_t& lo, uint64_t& hi,

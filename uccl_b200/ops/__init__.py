@@ -36,6 +36,10 @@ def all_reduce(tensor, op="sum", out=None, **kw):
     return default().all_reduce(tensor, op, out, **kw)
 
 
+def all_reduce_rmsnorm(x, residual, weight, eps=1e-6, **kw):
+    return default().all_reduce_rmsnorm(x, residual, weight, eps, **kw)
+
+
 def all_gather(out, tensor):
     return default().all_gather(out, tensor)
 

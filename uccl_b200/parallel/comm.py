@@ -72,6 +72,13 @@ def op_code(op) -> int:
         raise ValueError(f"uccl_b200: unsupported reduce op {op!r}") from e
 
 
+def _overlaps(a: torch.Tensor, b: torch.Tensor) -> bool:
+    """Do the storage byte ranges of two contiguous tensors intersect?"""
+    a0, b0 = a.data_ptr(), b.data_ptr()
+    a1, b1 = a0 + a.numel() * a.element_size(), b0 + b.numel() * b.element_size()
+    return a.device == b.device and a0 < b1 and b0 < a1
+
+
 class _HeapBlock:
     """Owns one symmetric-heap allocation; exposes it to torch without copying."""
 
@@ -242,6 +249,52 @@ class Communicator:
         self._c.allreduce(tensor.data_ptr(), out.data_ptr(), tensor.numel(), dtype_code(tensor.dtype), op_code(op),
                           self._stream(stream), a, float(scale), out_dt, max_ctas)
         return out
+
+    def all_reduce_rmsnorm(self, x: torch.Tensor, residual: torch.Tensor, weight: torch.Tensor, eps: float = 1e-6, *,
+                           residual_out: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+                           quant: Optional[str] = None, algo="auto", max_ctas: int = -1, stream=None):
+        """Sum all-reduce of ``x`` [T, H] in place, then ``residual_out = x + residual`` (over ``residual`` unless
+        given) and ``out = rmsnorm(residual_out, eps) * weight``; returns ``out``, or ``(out_e4m3, scales)`` with
+        ``quant="fp8"``.
+
+        The tail of every row-parallel layer of a tensor-parallel transformer in one call.  bf16 or fp16,
+        ``H % 8 == 0`` and ``H <= 16384`` (``H % 128 == 0`` for fp8).  Where the plain all-reduce would run one-shot
+        (small decode batches) everything is one kernel; larger ones run the selected all-reduce and then one
+        epilogue kernel.  Both paths give bitwise identical results on every rank.  The fp8 output is the
+        ``(x, scales)`` format of ``ep.utils.per_token_cast_to_fp8`` and ``ep.Buffer.dispatch``."""
+        for t, name in ((x, "x"), (residual, "residual"), (weight, "weight")):
+            self._check(t, name)
+        if x.dim() != 2:
+            raise ValueError("uccl_b200: all_reduce_rmsnorm x must be [tokens, hidden]")
+        T, H = x.shape
+        if residual.shape != x.shape or weight.shape != (H,) or residual.dtype != x.dtype or weight.dtype != x.dtype:
+            raise ValueError("uccl_b200: all_reduce_rmsnorm needs residual [T, H] and weight [H] of x's dtype")
+        if quant not in (None, "fp8"):
+            raise ValueError(f"uccl_b200: unsupported quant {quant!r} (None or 'fp8')")
+        if residual_out is None:
+            residual_out = residual
+        self._check(residual_out, "residual_out")
+        if residual_out.shape != x.shape or residual_out.dtype != x.dtype:
+            raise ValueError("uccl_b200: all_reduce_rmsnorm residual_out must match x")
+        fp8 = quant == "fp8"
+        out_dtype = torch.float8_e4m3fn if fp8 else x.dtype
+        if out is None:
+            out = torch.empty((T, H), dtype=out_dtype, device=x.device)
+        self._check(out, "out")
+        if out.shape != x.shape or out.dtype != out_dtype:
+            raise ValueError(f"uccl_b200: all_reduce_rmsnorm out must be [T, H] of {out_dtype}")
+        scales = torch.empty((T, H // 128), dtype=torch.float32, device=x.device) if fp8 else None
+        if _overlaps(out, x) or _overlaps(out, residual):
+            raise ValueError("uccl_b200: all_reduce_rmsnorm out must not alias x or residual")
+        if _overlaps(x, residual) or _overlaps(residual_out, x) or _overlaps(residual_out, out) or (
+                residual_out.data_ptr() != residual.data_ptr() and _overlaps(residual_out, residual)):
+            raise ValueError("uccl_b200: all_reduce_rmsnorm x, residual and residual_out must not overlap "
+                             "(residual_out may be residual itself)")
+        a = ALGOS[algo] if isinstance(algo, str) else int(algo)
+        self._c.allreduce_rmsnorm(x.data_ptr(), residual.data_ptr(), residual_out.data_ptr(), weight.data_ptr(),
+                                  out.data_ptr(), scales.data_ptr() if fp8 else 0, T, H, dtype_code(x.dtype),
+                                  float(eps), int(fp8), self._stream(stream), a, max_ctas)
+        return (out, scales) if fp8 else out
 
     def all_gather(self, out: torch.Tensor, tensor: torch.Tensor, stream=None) -> torch.Tensor:
         self._check(tensor, "tensor")
