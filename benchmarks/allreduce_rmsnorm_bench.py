@@ -12,6 +12,14 @@ max over ranks:
 Run without torchrun it uses one GPU: there is no communication, so it times the epilogue kernel
 (add_rmsnorm_kernel) against the torch tail and reports its achieved HBM bandwidth next to the H100 SXM data-sheet
 3.35 TB/s.  Virtual ranks on one GPU are not timed here: their kernels share one GPU's SMs and HBM.
+
+--mode sp times the sequence-parallel tail, reduce_scatter_rmsnorm, at prefill sizes (--tokens is the global T, a
+multiple of the world size; every rank normalises T / n rows):
+  fused    Communicator.reduce_scatter_rmsnorm (one kernel where the reduce-scatter runs the LL kernel)
+  unfused  our reduce_scatter, then x + residual, torch.nn.functional.rms_norm [, per_token_cast_to_fp8]
+  nccl     torch.distributed.reduce_scatter_tensor (NCCL), then the same torch tail
+Each row records which path the fused arm took ("path": fused / unfused, from the LL limit).  It needs torchrun with
+at least 2 ranks: on one GPU there is no communication to time, and --mode tp already times the epilogue kernel.
 """
 import argparse
 import json
@@ -48,13 +56,19 @@ def epilogue_bytes(T, H, fp8):
 
 def main():
     p = argparse.ArgumentParser()
-    p.add_argument("--tokens", default="1,4,16,64,256")
+    p.add_argument("--mode", choices=("tp", "sp"), default="tp",
+                   help="tp: all_reduce_rmsnorm at decode shapes; sp: reduce_scatter_rmsnorm at prefill shapes")
+    p.add_argument("--tokens", default=None, help="default 1,4,16,64,256 (tp) or 128,512,2048,8192 (sp, global T)")
     p.add_argument("--hidden", default="4096,7168,8192")
     p.add_argument("--iters", type=int, default=200)
     p.add_argument("--warmup", type=int, default=20)
     p.add_argument("--eps", type=float, default=1e-6)
     p.add_argument("--out", default=None)
     a = p.parse_args()
+    if a.tokens is None:
+        a.tokens = "128,512,2048,8192" if a.mode == "sp" else "1,4,16,64,256"
+    if a.mode == "sp" and int(os.environ.get("WORLD_SIZE", "1")) < 2:
+        sys.exit("--mode sp needs torchrun with at least 2 ranks: on one GPU there is no reduce-scatter to time")
 
     dist = None
     if "RANK" in os.environ:
@@ -102,8 +116,39 @@ def main():
 
     rows = []
     g = torch.Generator(device="cpu").manual_seed(rank)
+
+    def tail(x, res, w, H, fp8):
+        r = x + res
+        y = F.rms_norm(r, (H,), w, a.eps)
+        return per_token_cast_to_fp8(y) if fp8 else y
+
     for H in [int(v) for v in a.hidden.split(",")]:
         w = (torch.rand(H, generator=g) + 0.5).to(torch.bfloat16).to(dev)
+        if a.mode == "sp":
+            for T in [int(v) for v in a.tokens.split(",")]:
+                if T % n:
+                    raise SystemExit(f"--tokens: {T} is not a multiple of the world size {n}")
+                Tl = T // n
+                x0 = torch.randn(T, H, generator=g).to(torch.bfloat16).to(dev) * 0.01
+                res0 = torch.randn(Tl, H, generator=g).to(torch.bfloat16).to(dev)
+                x, res = x0.clone(), res0.clone()
+                xs = torch.empty(Tl, H, dtype=torch.bfloat16, device=dev)  # reduce-scatter output of the torch arms
+                for fp8 in (False, True):
+                    quant = "fp8" if fp8 else None
+                    nbytes = Tl * H * 2  # one rank's piece
+                    row = {"mode": "sp", "T": T, "rows_per_rank": Tl, "H": H, "fp8": fp8, "bytes_per_rank": nbytes,
+                           "n_gpus": n, "path": "fused" if nbytes <= comm.reduce_scatter_ll_max() else "unfused"}
+                    # x and residual are updated in place by every timed call; no arm's time depends on their values
+                    row["fused_us"] = timed(lambda: comm.reduce_scatter_rmsnorm(x, res, w, a.eps, quant=quant))
+                    row["unfused_us"] = timed(lambda: tail(comm.reduce_scatter(xs, x), res, w, H, fp8))
+                    x.copy_(x0)
+                    row["nccl_us"] = timed(lambda: (dist.reduce_scatter_tensor(xs, x), tail(xs, res, w, H, fp8)))
+                    x.copy_(x0)
+                    res.copy_(res0)
+                    rows.append(row)
+                    if rank == 0:
+                        print(json.dumps(row), flush=True)
+            continue
         for T in [int(v) for v in a.tokens.split(",")]:
             x0 = torch.randn(T, H, generator=g).to(torch.bfloat16).to(dev) * 0.01
             res0 = torch.randn(T, H, generator=g).to(torch.bfloat16).to(dev)
@@ -115,19 +160,14 @@ def main():
                 if n > 1:
                     row["fused_path"] = comm.select_allreduce(nbytes, comm.is_symmetric(x), torch.bfloat16)[0]
 
-                def tail(x, res):
-                    r = x + res
-                    y = F.rms_norm(r, (H,), w, a.eps)
-                    return per_token_cast_to_fp8(y) if fp8 else y
-
                 # x and residual are updated in place by every timed call; no arm's time depends on their values
                 row["fused_us"] = timed(lambda: comm.all_reduce_rmsnorm(x, res, w, a.eps, quant=quant))
                 if n > 1:
-                    row["unfused_us"] = timed(lambda: tail(comm.all_reduce(x, "sum"), res))
+                    row["unfused_us"] = timed(lambda: tail(comm.all_reduce(x, "sum"), res, w, H, fp8))
                     x.copy_(x0)
-                    row["nccl_us"] = timed(lambda: (dist.all_reduce(x), tail(x, res)))
+                    row["nccl_us"] = timed(lambda: (dist.all_reduce(x), tail(x, res, w, H, fp8)))
                 else:
-                    row["torch_tail_us"] = timed(lambda: tail(x, res))
+                    row["torch_tail_us"] = timed(lambda: tail(x, res, w, H, fp8))
                     row["epilogue_GBps"] = epilogue_bytes(T, H, fp8) / (row["fused_us"] * 1e-6) / 1e9
                     row["epilogue_share_of_hbm_peak"] = row["epilogue_GBps"] / HBM_PEAK_GBPS
                 x.copy_(x0)
@@ -135,9 +175,9 @@ def main():
                 rows.append(row)
                 if rank == 0:
                     print(json.dumps(row), flush=True)
-    result = {"n_gpus": n, "dtype": "bf16", "iters": a.iters, **info, "rows": rows}
+    result = {"mode": a.mode, "n_gpus": n, "dtype": "bf16", "iters": a.iters, **info, "rows": rows}
     if rank == 0:
-        print(json.dumps({"n_gpus": n, **info, "shapes": len(rows)}), flush=True)
+        print(json.dumps({"mode": a.mode, "n_gpus": n, **info, "shapes": len(rows)}), flush=True)
         if a.out:
             with open(a.out, "w") as f:
                 json.dump(result, f, indent=1)

@@ -131,6 +131,17 @@ PYBIND11_MODULE(_C, m) {
           py::arg("x"), py::arg("residual"), py::arg("residual_out"), py::arg("weight"), py::arg("out"),
           py::arg("out_scales"), py::arg("T"), py::arg("H"), py::arg("dtype"), py::arg("eps"), py::arg("quant"),
           py::arg("stream"), py::arg("algo") = 0, py::arg("max_ctas") = -1)
+      .def(
+          "reduce_scatter_rmsnorm",
+          [](Comm& c, uintptr_t x, uintptr_t residual, uintptr_t residual_out, uintptr_t weight, uintptr_t out,
+             uintptr_t out_scales, size_t T, size_t H, int dtype, float eps, int quant, uintptr_t stream) {
+            py::gil_scoped_release rel;
+            c.reduce_scatter_rmsnorm(P(x), P(residual), P(residual_out), P(weight), P(out),
+                                     reinterpret_cast<float*>(out_scales), T, H, dtype, eps, quant, S(stream));
+          },
+          py::arg("x"), py::arg("residual"), py::arg("residual_out"), py::arg("weight"), py::arg("out"),
+          py::arg("out_scales"), py::arg("T"), py::arg("H"), py::arg("dtype"), py::arg("eps"), py::arg("quant"),
+          py::arg("stream"))
       .def("allgather",
            [](Comm& c, uintptr_t in, uintptr_t out, size_t count, int dtype, uintptr_t stream) {
              py::gil_scoped_release rel;
@@ -188,6 +199,7 @@ PYBIND11_MODULE(_C, m) {
            py::arg("ops"), py::arg("stream") = 0)
       .def("set_tuning", &Comm::set_tuning)
       .def("set_xchg_ll_max", &Comm::set_xchg_ll_max)
+      .def("rs_ll_max_bytes", &Comm::rs_ll_max_bytes)
       .def("set_rs_push", &Comm::set_rs_push)
       .def("rs_push", &Comm::rs_push)
       .def("xchg_ll_max", &Comm::xchg_ll_max)

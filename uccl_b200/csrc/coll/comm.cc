@@ -351,6 +351,8 @@ static uint64_t xchg_ll_limit(int64_t v, int n, bool symmetric_push) {
   return std::min<uint64_t>(m, kLLMaxData);
 }
 
+uint64_t Comm::rs_ll_max_bytes() const { return nranks() > 1 ? xchg_ll_limit(xchg_ll_max_, nranks(), false) : 0; }
+
 // ------------------------------------------------------------------ allreduce
 void Comm::allreduce(const void* in, void* out, size_t count, int dtype, int op, cudaStream_t stream,
                      const ArOpts& opts) {
@@ -538,6 +540,73 @@ void Comm::allreduce_rmsnorm(void* x, const void* residual, void* residual_out, 
   UB_CHECK(e == cudaSuccess, "add_rmsnorm launch failed (rank %d): %s", rank(), cudaGetErrorString(e));
   ++launches_;
   UB_TRACE(SUB_COLL, "allreduce_rmsnorm unfused T=%zu H=%zu algo=%s", T, H, algo_name(algo));
+}
+
+// ------------------------------------------------------ reduce_scatter + rmsnorm
+void Comm::reduce_scatter_rmsnorm(void* x, const void* residual, void* residual_out, const void* weight, void* out,
+                                  float* out_scales, size_t T, size_t H, int dtype, float eps, int quant,
+                                  cudaStream_t stream) {
+  UB_CHECK(dtype == kBF16 || dtype == kF16, "reduce_scatter_rmsnorm: dtype must be bf16 or fp16 (got %d)", dtype);
+  UB_CHECK(H >= 8 && H <= kRmsMaxH && H % 8 == 0,
+           "reduce_scatter_rmsnorm: hidden size %zu must be a multiple of 8 in [8, %u]", H, kRmsMaxH);
+  UB_CHECK(quant == 0 || quant == 1, "reduce_scatter_rmsnorm: bad quant %d", quant);
+  UB_CHECK(!quant || H % 128 == 0, "reduce_scatter_rmsnorm: fp8 output needs hidden size %% 128 == 0 (got %zu)", H);
+  UB_CHECK(T <= UINT32_MAX, "reduce_scatter_rmsnorm: too many rows (%zu)", T);
+  const int n = nranks();
+  UB_CHECK(T % n == 0, "reduce_scatter_rmsnorm: %zu tokens do not split evenly over %d ranks", T, n);
+  if (T == 0) return;
+  check_buf(x, "x");
+  check_buf(residual, "residual");
+  check_buf(residual_out, "residual_out");
+  check_buf(weight, "weight");
+  check_buf(out, "out");
+  if (quant) check_buf(out_scales, "out_scales");
+  float* scales = quant ? out_scales : nullptr;
+  const size_t Tl = T / n, count = Tl * H, bytes = count * dtype_size(dtype);  // one rank's piece
+  char* own = static_cast<char*>(x) + (size_t)rank() * bytes;
+  if (is_host()) {
+    host_reduce_scatter(x, own, count, dtype, kSum);  // stages every piece before it reduces: in place is safe
+    host_add_rmsnorm(own, residual, residual_out, weight, out, scales, Tl, H, dtype, eps);
+    return;
+  }
+  DeviceGuard g(device());
+  UB_CHECK(aligned16(x) && aligned16(residual) && aligned16(residual_out) && aligned16(weight) && aligned16(out),
+           "reduce_scatter_rmsnorm: x, residual, residual_out, weight and out must be 16-byte aligned");
+  RmsNormArgs r;
+  r.x = own;
+  r.residual = residual;
+  r.residual_out = residual_out;
+  r.weight = weight;
+  r.out = out;
+  r.out_scales = scales;
+  r.T = (uint32_t)Tl;
+  r.H = (uint32_t)H;
+  r.eps = eps;
+
+  // the fused kernel takes exactly the sizes for which the plain reduce_scatter would run the LL kernel
+  // (bytes % 16 == 0 because H % 8 == 0), with that kernel's grid
+  if (bytes <= rs_ll_max_bytes()) {
+    const int ctas = ctas_for(bytes * (uint64_t)(n - 1), std::min(max_ctas_, 64), 16 << 10);
+    CollArgs a = base_args();
+    a.in = x;
+    a.out = own;
+    a.bytes = bytes;
+    a.count = count;
+    cudaError_t e = launch_reduce_scatter_rmsnorm(dtype, quant != 0, dev_, a, r, ctas, stream);
+    UB_CHECK(e == cudaSuccess, "reduce_scatter_rmsnorm launch failed (rank %d ctas=%d): %s", rank(), ctas,
+             cudaGetErrorString(e));
+    ++launches_;
+    UB_TRACE(SUB_COLL, "reduce_scatter_rmsnorm fused T=%zu H=%zu ctas=%d", T, H, ctas);
+    return;
+  }
+  // in place: every reduce_scatter kernel reads the own piece of its input before (or, per unit, as) it writes the
+  // result over it, and peers only read their own pieces (see rs_kernel)
+  if (n > 1) reduce_scatter(x, own, count, dtype, kSum, stream);
+  const int grid = (int)std::min<size_t>(Tl, 1024);
+  cudaError_t e = launch_allreduce_rmsnorm(0, dtype, quant != 0, dev_, base_args(), r, grid, stream);
+  UB_CHECK(e == cudaSuccess, "add_rmsnorm launch failed (rank %d): %s", rank(), cudaGetErrorString(e));
+  ++launches_;
+  UB_TRACE(SUB_COLL, "reduce_scatter_rmsnorm unfused T=%zu H=%zu", T, H);
 }
 
 // ------------------------------------------------------------------ allgather

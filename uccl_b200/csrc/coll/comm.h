@@ -99,6 +99,13 @@ class Comm {
   void allreduce_rmsnorm(void* x, const void* residual, void* residual_out, const void* weight, void* out,
                          float* out_scales, size_t T, size_t H, int dtype, float eps, int quant, cudaStream_t stream,
                          const ArOpts& opts = ArOpts());
+  // Sequence-parallel counterpart: x [T, H] (T % nranks == 0) is sum-reduce-scattered in place, so that rank r's row
+  // block x[r*T/n, (r+1)*T/n) holds its rows of the sum; then the same epilogue on that block with residual,
+  // residual_out, out [T/n, H] and out_scales [T/n, H / 128].  The fused LL kernel runs where the plain
+  // reduce_scatter of T/n * H elements would take the LL kernel; otherwise reduce_scatter, then the epilogue kernel.
+  void reduce_scatter_rmsnorm(void* x, const void* residual, void* residual_out, const void* weight, void* out,
+                              float* out_scales, size_t T, size_t H, int dtype, float eps, int quant,
+                              cudaStream_t stream);
   // grouped point-to-point (ncclGroupStart .. ncclSend/ncclRecv .. ncclGroupEnd)
   struct P2pOp {
     bool is_send;
@@ -114,6 +121,8 @@ class Comm {
   // LL-packet AllGather/AllToAll/ReduceScatter threshold (per-rank piece bytes): 0 default, <0 off
   void set_xchg_ll_max(int64_t bytes) { xchg_ll_max_ = bytes; }
   int64_t xchg_ll_max() const { return xchg_ll_max_; }
+  // per-rank piece size up to which reduce_scatter and reduce_scatter_rmsnorm run the LL kernels (0: never)
+  uint64_t rs_ll_max_bytes() const;
   // staged (plain-buffer) ReduceScatter: push pieces into the peers' stages instead of copy-in + pull.
   // Must be set identically on every rank.
   void set_rs_push(bool on) { rs_push_ = on; }

@@ -57,6 +57,8 @@ cudaError_t preload_all_kernels() {
     for (int algo : {0, 1, 2})
       for (int dt : {(int)kBF16, (int)kF16})
         for (bool fp8 : {false, true}) ok(launch_allreduce_rmsnorm(algo, dt, fp8, c, a, r, 1, 0));
+    for (int dt : {(int)kBF16, (int)kF16})
+      for (bool fp8 : {false, true}) ok(launch_reduce_scatter_rmsnorm(dt, fp8, c, a, r, 1, 0));
   }
   for (int m = 0; m < 5; ++m) ok(launch_allgather(m, c, a, 1, 512, 0));
   for (int m = 0; m < 4; ++m) ok(launch_broadcast(m, c, a, 1, 512, 0));

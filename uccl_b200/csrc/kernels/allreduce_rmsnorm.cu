@@ -9,10 +9,15 @@
 //                                   publishes and reduces rows b, b + grid, ... and runs the row epilogue on the
 //                                   reduced row while it is still in registers.  No barrier, no extra HBM pass.
 //   add_rmsnorm_kernel<T, FP8>      the same row epilogue on an already reduced x (the unfused path behind the
-//                                   two-shot / staged / NVLS all-reduce, and one-rank communicators).
-// Both run the identical epilogue with the identical thread -> element mapping, so their results are bitwise equal.
+//                                   two-shot / staged / NVLS all-reduce or the barrier-based reduce-scatter, and
+//                                   one-rank communicators).
+//   rs_ll_rmsnorm<T, FP8>           sequence-parallel variant: the LL reduce-scatter of ll_exchange.cuh with a
+//                                   row-owned phase 2; x is [T, H] summed over ranks, and rank r keeps, reduces and
+//                                   normalises only its T / n rows (residual, residual_out and out are that shard).
+// All run the identical epilogue with the identical thread -> element mapping, so their results are bitwise equal.
 #include "allreduce_impl.cuh"
 #include "fp8_quant.cuh"
+#include "ll_exchange.cuh"
 
 namespace ub {
 
@@ -165,6 +170,51 @@ __global__ void __launch_bounds__(kRmsThreads) add_rmsnorm_kernel(const __grid_c
   }
 }
 
+// Fused sequence-parallel path: rs_ll_kernel's phases and protocol (ll_begin / ll_end of ll_exchange.cuh: the same
+// epoch words and parity slots as every other LL collective and the one-shot all-reduce).  a.in = the whole x,
+// a.bytes = one rank's piece (r.T * H * sizeof(T), with r.T = T / n rows); r.x = my own piece of x.
+// Phase 1 pushes the peers' pieces and never reads my own, so phase 2 may store the sum over it: every unit of my
+// piece is loaded and stored by one thread only.  Blocks past the last row only push: the grid is rs_ll_kernel's,
+// which keeps phase 1 wide when a rank has one or two rows, and never exceeds it (co-residency of virtual ranks).
+template <typename T, bool FP8>
+__global__ void __launch_bounds__(kRmsThreads) rs_ll_rmsnorm(const __grid_constant__ DevComm c,
+                                                             const __grid_constant__ CollArgs a,
+                                                             const __grid_constant__ RmsNormArgs r) {
+  __shared__ float s_warp[kRmsThreads / 32];
+  const LLCtx l = ll_begin(c, a);
+  const uint32_t upr = r.H / 8;
+  const int n = c.nranks, rank = c.rank, tid = threadIdx.x;
+
+  ll_scatter_pieces(c, a, l, (uint64_t)r.T * upr);
+
+  const char* my_ll = c.heap[rank] + l.parity_off;
+  char* x = static_cast<char*>(r.x);
+  for (uint64_t row = blockIdx.x; row < r.T; row += gridDim.x) {
+    float v[kRmsUnits][8];
+#pragma unroll
+    for (int k = 0; k < kRmsUnits; ++k) {
+      const uint32_t ur = k * kRmsThreads + tid;
+      if (ur >= upr) continue;
+      const uint64_t u = row * upr + ur;  // unit of my piece = unit of every peer's packet slot
+      Vec16<T, kSum> acc;
+      for (int s = 0; s < n; ++s) {
+        const uint4 d =
+            s == rank ? ld_v4(x + u * 16) : ll_get(c, my_ll + (uint64_t)s * kLLSlotBytes + u * 32, l.flag, s);
+        if (s == 0) acc.init(d);
+        else acc.accum(d);
+      }
+      const uint4 sum = acc.pack_same();
+      st_v4(x + u * 16, sum);
+      Vec16<T, kSum> rounded;
+      rounded.init(sum);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) v[k][i] = rounded.a[i];
+    }
+    rmsnorm_row<T, FP8>(v, row, r, s_warp);
+  }
+  ll_end(l);
+}
+
 template <typename T, bool FP8>
 static cudaError_t launch_rms_typed(int algo, const DevComm& c, const CollArgs& a, const RmsNormArgs& r, int grid,
                                     cudaStream_t st) {
@@ -188,6 +238,22 @@ cudaError_t launch_allreduce_rmsnorm(int algo, int dtype, bool fp8, const DevCom
                  : launch_rms_typed<__half, false>(algo, c, a, r, grid, st);
     default: return cudaErrorInvalidValue;
   }
+}
+
+cudaError_t launch_reduce_scatter_rmsnorm(int dtype, bool fp8, const DevComm& c, const CollArgs& a,
+                                          const RmsNormArgs& r, int grid, cudaStream_t st) {
+  switch (dtype) {
+    case kBF16:
+      if (fp8) UB_LAUNCH((rs_ll_rmsnorm<__nv_bfloat16, true>), grid, kRmsThreads, 0, st, c, a, r);
+      else UB_LAUNCH((rs_ll_rmsnorm<__nv_bfloat16, false>), grid, kRmsThreads, 0, st, c, a, r);
+      break;
+    case kF16:
+      if (fp8) UB_LAUNCH((rs_ll_rmsnorm<__half, true>), grid, kRmsThreads, 0, st, c, a, r);
+      else UB_LAUNCH((rs_ll_rmsnorm<__half, false>), grid, kRmsThreads, 0, st, c, a, r);
+      break;
+    default: return cudaErrorInvalidValue;
+  }
+  return cudaGetLastError();
 }
 
 }  // namespace ub

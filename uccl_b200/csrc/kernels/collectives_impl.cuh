@@ -159,6 +159,11 @@ __global__ void __launch_bounds__(512, 1) ag_kernel(const __grid_constant__ DevC
 // ------------------------------------------------------------- ReduceScatter
 // a.count = elements each rank receives; input holds n * count elements of T.
 // NVLS requires a symmetric input. Output is a plain local buffer.
+// In place (out = in + rank * bytes, NCCL's in-place reduce-scatter; reduce_scatter_rmsnorm relies on it) is safe in
+// every variant.  Push: block b writes its slice of a chunk only after the barrier that follows its own push of that
+// slice of every piece, own piece included, and later chunks read other bytes.  Pull / zero-copy: peer q only reads
+// piece q of my input (or of my stage, which holds a copy made before the barrier), never my own piece, and each
+// thread reads my own units before it stores their sum.
 template <typename T, int OP, bool NVLS>
 __global__ void __launch_bounds__(512, 1) rs_kernel(const __grid_constant__ DevComm c,
                                                     const __grid_constant__ CollArgs a) {

@@ -36,6 +36,11 @@ cudaError_t launch_allreduce_x(int algo, int dtype, int op, const DevComm& c, co
 // already reduced r.x.  dtype kBF16 / kF16; fp8 = e4m3 output with per-128-channel scales.
 cudaError_t launch_allreduce_rmsnorm(int algo, int dtype, bool fp8, const DevComm& c, const CollArgs& a,
                                      const RmsNormArgs& r, int grid, cudaStream_t st);
+// LL reduce-scatter (sum) + residual add + RMSNorm [+ e4m3 cast] (allreduce_rmsnorm.cu): a = LL reduce-scatter
+// arguments with in = the whole x and bytes = one rank's piece; r = this rank's shard (r.x = its piece of x, r.T = its
+// rows).  Block size kRmsThreads; bytes % 16 == 0.
+cudaError_t launch_reduce_scatter_rmsnorm(int dtype, bool fp8, const DevComm& c, const CollArgs& a,
+                                          const RmsNormArgs& r, int grid, cudaStream_t st);
 // allgather modes: 0 push P2P, 1 push multicast, 2 pull/staged, 3 LL packets, 4 LL packets via multicast
 cudaError_t launch_allgather(int mode, const DevComm& c, const CollArgs& a, int grid, int block, cudaStream_t st);
 cudaError_t launch_broadcast(int mode, const DevComm& c, const CollArgs& a, int grid, int block, cudaStream_t st);

@@ -40,6 +40,10 @@ def all_reduce_rmsnorm(x, residual, weight, eps=1e-6, **kw):
     return default().all_reduce_rmsnorm(x, residual, weight, eps, **kw)
 
 
+def reduce_scatter_rmsnorm(x, residual, weight, eps=1e-6, **kw):
+    return default().reduce_scatter_rmsnorm(x, residual, weight, eps, **kw)
+
+
 def all_gather(out, tensor):
     return default().all_gather(out, tensor)
 

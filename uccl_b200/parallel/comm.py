@@ -296,6 +296,63 @@ class Communicator:
                                   float(eps), int(fp8), self._stream(stream), a, max_ctas)
         return (out, scales) if fp8 else out
 
+    def reduce_scatter_rmsnorm(self, x: torch.Tensor, residual: torch.Tensor, weight: torch.Tensor,
+                               eps: float = 1e-6, *, residual_out: Optional[torch.Tensor] = None,
+                               out: Optional[torch.Tensor] = None, quant: Optional[str] = None, stream=None):
+        """Sequence-parallel layer tail: reduce-scatter ``x`` [T, H] over tokens, then add + RMSNorm this rank's rows.
+
+        The tail of a row-parallel layer with sequence parallelism in one call.  Returns ``out`` [T/n, H], or
+        ``(out_e4m3, scales)`` with ``quant="fp8"``.
+
+        With ``n`` ranks, rank ``r`` and ``Tl = T / n`` (``T % n == 0``): ``x[r*Tl:(r+1)*Tl]`` becomes this rank's
+        rows of the sum over ranks, in place as NCCL's in-place reduce-scatter (the rest of ``x`` is unchanged);
+        ``residual`` [Tl, H] is this rank's shard, rows ``r*Tl .. (r+1)*Tl`` of the full residual;
+        ``residual_out = x[r*Tl:(r+1)*Tl] + residual`` (over ``residual`` unless given) and
+        ``out = rmsnorm(residual_out, eps) * weight``.  bf16 or fp16, ``H % 8 == 0`` and ``H <= 16384``
+        (``H % 128 == 0`` for fp8).  Where the plain reduce-scatter of one rank's rows would run the LL kernel
+        everything is one kernel; larger ones run the reduce-scatter and then one epilogue kernel.  Both paths, and
+        the ranks' shards concatenated in rank order, give bitwise what :meth:`all_reduce_rmsnorm` gives on the same
+        ``x`` and the full residual.  The fp8 output is the ``(x, scales)`` format of
+        ``ep.utils.per_token_cast_to_fp8``; the full ``[T, H]`` pair for the next column-parallel layer is two plain
+        :meth:`all_gather` calls, one of ``out_e4m3`` and one of ``scales``."""
+        for t, name in ((x, "x"), (residual, "residual"), (weight, "weight")):
+            self._check(t, name)
+        if x.dim() != 2:
+            raise ValueError("uccl_b200: reduce_scatter_rmsnorm x must be [tokens, hidden]")
+        T, H = x.shape
+        n = self.world_size
+        if T % n:
+            raise ValueError(f"uccl_b200: reduce_scatter_rmsnorm needs tokens ({T}) divisible by the world size ({n})")
+        Tl = T // n
+        if residual.shape != (Tl, H) or weight.shape != (H,) or residual.dtype != x.dtype or weight.dtype != x.dtype:
+            raise ValueError("uccl_b200: reduce_scatter_rmsnorm needs residual [T / world_size, H] and weight [H] "
+                             "of x's dtype")
+        if quant not in (None, "fp8"):
+            raise ValueError(f"uccl_b200: unsupported quant {quant!r} (None or 'fp8')")
+        if residual_out is None:
+            residual_out = residual
+        self._check(residual_out, "residual_out")
+        if residual_out.shape != (Tl, H) or residual_out.dtype != x.dtype:
+            raise ValueError("uccl_b200: reduce_scatter_rmsnorm residual_out must match residual")
+        fp8 = quant == "fp8"
+        out_dtype = torch.float8_e4m3fn if fp8 else x.dtype
+        if out is None:
+            out = torch.empty((Tl, H), dtype=out_dtype, device=x.device)
+        self._check(out, "out")
+        if out.shape != (Tl, H) or out.dtype != out_dtype:
+            raise ValueError(f"uccl_b200: reduce_scatter_rmsnorm out must be [T / world_size, H] of {out_dtype}")
+        scales = torch.empty((Tl, H // 128), dtype=torch.float32, device=x.device) if fp8 else None
+        if _overlaps(out, x) or _overlaps(out, residual):
+            raise ValueError("uccl_b200: reduce_scatter_rmsnorm out must not alias x or residual")
+        if _overlaps(x, residual) or _overlaps(residual_out, x) or _overlaps(residual_out, out) or (
+                residual_out.data_ptr() != residual.data_ptr() and _overlaps(residual_out, residual)):
+            raise ValueError("uccl_b200: reduce_scatter_rmsnorm x, residual and residual_out must not overlap "
+                             "(residual_out may be residual itself)")
+        self._c.reduce_scatter_rmsnorm(x.data_ptr(), residual.data_ptr(), residual_out.data_ptr(), weight.data_ptr(),
+                                       out.data_ptr(), scales.data_ptr() if fp8 else 0, T, H, dtype_code(x.dtype),
+                                       float(eps), int(fp8), self._stream(stream))
+        return (out, scales) if fp8 else out
+
     def all_gather(self, out: torch.Tensor, tensor: torch.Tensor, stream=None) -> torch.Tensor:
         self._check(tensor, "tensor")
         self._check(out, "out")
@@ -480,6 +537,11 @@ class Communicator:
         """Per-rank piece size up to which all_gather / all_to_all / reduce_scatter use the barrier-free
         LL-packet kernels (0: built-in default per world size, negative: never)."""
         self._c.set_xchg_ll_max(int(nbytes))
+
+    def reduce_scatter_ll_max(self) -> int:
+        """Per-rank piece size (bytes) up to which reduce_scatter runs the LL-packet kernel, and
+        reduce_scatter_rmsnorm its fused kernel (0: never, e.g. on one rank)."""
+        return int(self._c.rs_ll_max_bytes())
 
 
 def launch_count(comms: Iterable[Communicator]) -> int:
