@@ -20,6 +20,16 @@ multiple of the world size; every rank normalises T / n rows):
   nccl     torch.distributed.reduce_scatter_tensor (NCCL), then the same torch tail
 Each row records which path the fused arm took ("path": fused / unfused, from the LL limit).  It needs torchrun with
 at least 2 ranks: on one GPU there is no communication to time, and --mode tp already times the epilogue kernel.
+
+--mode ep times the tail of an expert-parallel MoE layer, ep.Buffer.combine_rmsnorm, with the routing of bench.py (top-8
+of 256 experts, --tokens per rank, default 128,512,4096 at H = 7168), bf16 and fp8 out, and config.num_sms of 24 and of
+every SM:
+  fused    Buffer.combine_rmsnorm (one kernel)
+  unfused  Buffer.combine, then add_rmsnorm_kernel (all_reduce_rmsnorm of a one-rank communicator)
+  torch    Buffer.combine, then x + residual, torch.nn.functional.rms_norm [, per_token_cast_to_fp8]
+Fused and unfused outputs are checked bitwise equal first.  The arms' graphs are replayed alternately --rounds times;
+each row reports the median, min and max per call, the bytes moved (from shapes) and the achieved rate next to the
+3.35 TB/s data sheet.  It runs on one GPU without torchrun (no NVLink traffic, HBM-bound) and under torchrun for n >= 2.
 """
 import argparse
 import json
@@ -54,19 +64,143 @@ def epilogue_bytes(T, H, fp8):
     return 3 * T * H * 2 + H * 2 + out
 
 
+def combine_bytes(T, num_recv, H):
+    """HBM traffic of Buffer.combine without bias: read the expert rows, write the combined rows."""
+    return num_recv * H * 2 + T * H * 2
+
+
+def ep_fused_bytes(T, num_recv, H, fp8):
+    """combine_rmsnorm: read the expert rows, residual and weight; write residual_out and out (+ scales)."""
+    return combine_bytes(T, num_recv, H) + epilogue_bytes(T, H, fp8) - 2 * T * H * 2
+
+
+def run_ep(a, rank, n, dev, dist, info):
+    """--mode ep: see the module docstring."""
+    from uccl_b200.ep import Buffer, Config
+
+    H, K, E = [int(v) for v in a.hidden.split(",")][0], 8, 256
+    tokens = [int(v) for v in a.tokens.split(",")]
+    T_max = max(tokens)
+    nvl = Config().get_nvl_buffer_size_hint(H * 2, n, T_max, K)
+    if dist is not None:
+        comm = Communicator.from_torch_dist(None, heap_bytes=nvl + (256 << 20), stage_bytes=16 << 20)
+    else:
+        comm = Communicator.local_world(1, devices=[dev.index], heap_bytes=nvl + (256 << 20), stage_bytes=16 << 20)[0]
+    buf = Buffer(comm=comm, num_nvl_bytes=nvl)
+    one = Communicator.local_world(1, devices=[dev.index], heap_bytes=256 << 20, stage_bytes=8 << 20)[0]
+    all_sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    g = torch.Generator(device="cpu").manual_seed(rank)
+    w = (torch.rand(H, generator=g) + 0.5).to(torch.bfloat16).to(dev)
+    rows = []
+
+    def graph_of(fn):
+        for _ in range(a.warmup):
+            fn()
+        torch.cuda.synchronize()
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            for _ in range(a.iters):
+                fn()
+        graph.replay()
+        torch.cuda.synchronize()
+        return graph
+
+    def replay_us(graph):
+        if dist is not None:
+            dist.barrier()
+        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        s.record()
+        graph.replay()
+        e.record()
+        torch.cuda.synchronize()
+        return mx(s.elapsed_time(e) / a.iters * 1e3, dist, dev)
+
+    for T in tokens:
+        x = torch.randn(T, H, generator=g).to(torch.bfloat16).to(dev)
+        idx = torch.rand(T, E, generator=g).topk(K, dim=1).indices.to(torch.int64).to(dev)
+        tpr, _, tpe, in_rank, _ = buf.get_dispatch_layout(idx, E)
+        recv_x, _, _, _, handle, _ = buf.dispatch(x, num_tokens_per_rank=tpr, is_token_in_rank=in_rank,
+                                                  num_tokens_per_expert=tpe, topk_idx=idx)
+        num_recv = recv_x.size(0)
+        cb = buf.get_combine_buffer(num_recv, H)
+        cb.copy_(recv_x)
+        res = torch.randn(T, H, generator=g).to(torch.bfloat16).to(dev)
+        torch.cuda.synchronize()
+        for sms in (24, all_sms):
+            cfg = Config(sms)
+            for fp8 in (False, True):
+                quant = "fp8" if fp8 else None
+                ro_f, ro_u = torch.empty_like(res), torch.empty_like(res)  # residual stays the input of every call
+
+                def fused():
+                    return buf.combine_rmsnorm(cb, handle, res, w, a.eps, residual_out=ro_f, quant=quant, config=cfg)[0]
+
+                def unfused():
+                    c = buf.combine(cb, handle, config=cfg)[0]
+                    return one.all_reduce_rmsnorm(c, res, w, a.eps, residual_out=ro_u, quant=quant)
+
+                def torch_tail():
+                    c = buf.combine(cb, handle, config=cfg)[0]
+                    y = F.rms_norm(c + res, (H,), w, a.eps)
+                    return per_token_cast_to_fp8(y) if fp8 else y
+
+                yf, yu = fused(), unfused()
+                torch.cuda.synchronize()
+                same = torch.equal(ro_f, ro_u) and all(
+                    torch.equal(p.view(torch.uint8), q.view(torch.uint8))
+                    for p, q in zip(yf if fp8 else (yf,), yu if fp8 else (yu,)))
+                if not same:
+                    raise SystemExit(f"--mode ep: fused and unfused outputs differ (T={T}, num_sms={sms}, fp8={fp8})")
+                graphs = {"fused": graph_of(fused), "unfused": graph_of(unfused), "torch": graph_of(torch_tail)}
+                times = {k: [] for k in graphs}
+                for _ in range(a.rounds):  # alternate the arms so drift and neighbours hit them alike
+                    for k, gr in graphs.items():
+                        times[k].append(replay_us(gr))
+                del graphs
+                row = {"mode": "ep", "T": T, "num_recv": num_recv, "H": H, "topk": K, "experts": E, "fp8": fp8,
+                       "num_sms": sms, "n_gpus": n, "bitwise_fused_eq_unfused": same}
+                for k, v in times.items():
+                    v = sorted(v)
+                    row[f"{k}_us"] = v[len(v) // 2]
+                    row[f"{k}_us_min"], row[f"{k}_us_max"] = v[0], v[-1]
+                row["fused_bytes"] = ep_fused_bytes(T, num_recv, H, fp8)
+                row["unfused_bytes"] = combine_bytes(T, num_recv, H) + epilogue_bytes(T, H, fp8)
+                for k in ("fused", "unfused"):
+                    row[f"{k}_GBps"] = row[f"{k}_bytes"] / (row[f"{k}_us"] * 1e-6) / 1e9
+                    row[f"{k}_share_of_hbm_peak"] = row[f"{k}_GBps"] / HBM_PEAK_GBPS
+                row["speedup_vs_unfused"] = row["unfused_us"] / row["fused_us"]
+                rows.append(row)
+                if rank == 0:
+                    print(json.dumps(row), flush=True)
+    return rows
+
+
+def mx(v, dist, dev):
+    if dist is None:
+        return v
+    t = torch.tensor([v], dtype=torch.float64, device=dev)
+    dist.all_reduce(t, op=dist.ReduceOp.MAX)
+    return float(t.item())
+
+
 def main():
     p = argparse.ArgumentParser()
-    p.add_argument("--mode", choices=("tp", "sp"), default="tp",
-                   help="tp: all_reduce_rmsnorm at decode shapes; sp: reduce_scatter_rmsnorm at prefill shapes")
-    p.add_argument("--tokens", default=None, help="default 1,4,16,64,256 (tp) or 128,512,2048,8192 (sp, global T)")
-    p.add_argument("--hidden", default="4096,7168,8192")
+    p.add_argument("--mode", choices=("tp", "sp", "ep"), default="tp",
+                   help="tp: all_reduce_rmsnorm at decode shapes; sp: reduce_scatter_rmsnorm at prefill shapes; "
+                        "ep: ep.Buffer.combine_rmsnorm at bench.py's MoE routing")
+    p.add_argument("--tokens", default=None,
+                   help="default 1,4,16,64,256 (tp), 128,512,2048,8192 (sp, global T) or 128,512,4096 (ep, per rank)")
+    p.add_argument("--hidden", default=None, help="default 4096,7168,8192 (tp, sp) or 7168 (ep, first value used)")
+    p.add_argument("--rounds", type=int, default=5, help="ep: alternating replays of each arm's graph")
     p.add_argument("--iters", type=int, default=200)
     p.add_argument("--warmup", type=int, default=20)
     p.add_argument("--eps", type=float, default=1e-6)
     p.add_argument("--out", default=None)
     a = p.parse_args()
     if a.tokens is None:
-        a.tokens = "128,512,2048,8192" if a.mode == "sp" else "1,4,16,64,256"
+        a.tokens = {"sp": "128,512,2048,8192", "ep": "128,512,4096"}.get(a.mode, "1,4,16,64,256")
+    if a.hidden is None:
+        a.hidden = "7168" if a.mode == "ep" else "4096,7168,8192"
     if a.mode == "sp" and int(os.environ.get("WORLD_SIZE", "1")) < 2:
         sys.exit("--mode sp needs torchrun with at least 2 ranks: on one GPU there is no reduce-scatter to time")
 
@@ -78,13 +212,27 @@ def main():
         torch.cuda.set_device(local)
         dev = torch.device("cuda", local)
         dist.init_process_group("cpu:gloo,cuda:nccl", device_id=dev)
-        comm = Communicator.from_torch_dist(None, heap_bytes=512 << 20, stage_bytes=64 << 20)
     else:
         rank, n = 0, 1
         torch.cuda.set_device(0)
         dev = torch.device("cuda", 0)
-        comm = Communicator.local_world(1, devices=[0], heap_bytes=512 << 20, stage_bytes=64 << 20)[0]
     info = card()
+    if a.mode == "ep":
+        rows = run_ep(a, rank, n, dev, dist, info)
+        if rank == 0:
+            print(json.dumps({"mode": "ep", "n_gpus": n, **info, "shapes": len(rows)}), flush=True)
+            if a.out:
+                with open(a.out, "w") as f:
+                    json.dump({"mode": "ep", "n_gpus": n, "dtype": "bf16", "iters": a.iters, "rounds": a.rounds, **info,
+                               "rows": rows}, f, indent=1)
+        if dist is not None:
+            dist.barrier()
+            dist.destroy_process_group()
+        return
+    if dist is not None:
+        comm = Communicator.from_torch_dist(None, heap_bytes=512 << 20, stage_bytes=64 << 20)
+    else:
+        comm = Communicator.local_world(1, devices=[0], heap_bytes=512 << 20, stage_bytes=64 << 20)[0]
 
     def mx(v):
         if dist is None:

@@ -40,6 +40,20 @@ PYBIND11_MODULE(_C, m) {
   m.def("dtype_size", [](int dt) { return dtype_size(dt); });
   m.def("algo_name", [](int a) { return std::string(algo_name(a)); });
   m.def("param", [](const std::string& name, int64_t dflt) { return param_load(name.c_str(), dflt); });
+  // the CPU epilogue of the fused layer tails on an already reduced x (host memory): the host EP backend's
+  // combine_rmsnorm runs its own combine, then this
+  m.def(
+      "host_add_rmsnorm",
+      [](uintptr_t x, uintptr_t residual, uintptr_t residual_out, uintptr_t weight, uintptr_t out, uintptr_t out_scales,
+         size_t T, size_t H, int dtype, float eps) {
+        UB_CHECK(dtype == kBF16 || dtype == kF16, "host_add_rmsnorm: dtype must be bf16 or fp16 (got %d)", dtype);
+        UB_CHECK(!out_scales || H % 128 == 0, "host_add_rmsnorm: fp8 output needs hidden size %% 128 == 0");
+        py::gil_scoped_release rel;
+        host_add_rmsnorm(P(x), P(residual), P(residual_out), P(weight), P(out), reinterpret_cast<float*>(out_scales), T,
+                         H, dtype, eps);
+      },
+      py::arg("x"), py::arg("residual"), py::arg("residual_out"), py::arg("weight"), py::arg("out"),
+      py::arg("out_scales"), py::arg("T"), py::arg("H"), py::arg("dtype"), py::arg("eps"));
 
   py::class_<TuneEntry>(m, "TuneEntry")
       .def(py::init([](uint64_t max_bytes, int algo, int ctas) { return TuneEntry{max_bytes, algo, ctas}; }))

@@ -107,6 +107,14 @@ cudaError_t preload_all_kernels() {
     ok(launch_ep_combine(cn, ca, 1, 0));
     ca.bias0 = &dummy_bias;
     ok(launch_ep_combine(cn, ca, 1, 0));
+    RmsNormArgs r;
+    memset(&r, 0, sizeof(r));
+    for (bool fp8 : {false, true}) {
+      ca.bias0 = nullptr;
+      ok(launch_ep_combine_rmsnorm(cn, ca, r, fp8, 1, 0));
+      ca.bias0 = &dummy_bias;
+      ok(launch_ep_combine_rmsnorm(cn, ca, r, fp8, 1, 0));
+    }
   }
   {
     DevComm cn = c;

@@ -107,7 +107,17 @@ void bind_ep(py::module_& m) {
       .def("combine", [](EpBuffer& b, uintptr_t x, int num_recv, uintptr_t tw, uintptr_t ss, uintptr_t b0,
                          uintptr_t b1, uintptr_t out, uintptr_t otw, int T, int H, int K, int num_sms, uintptr_t st) {
         b.combine(x, num_recv, tw, ss, b0, b1, out, otw, T, H, K, num_sms, (cudaStream_t)st);
-      });
+      })
+      .def("combine_rmsnorm",
+           [](EpBuffer& b, uintptr_t x, int num_recv, uintptr_t ss, uintptr_t b0, uintptr_t b1, uintptr_t residual,
+              uintptr_t residual_out, uintptr_t weight, uintptr_t out, uintptr_t out_scales, int T, int H, float eps,
+              int num_sms, uintptr_t st) {
+             b.combine_rmsnorm(x, num_recv, ss, b0, b1, residual, residual_out, weight, out, out_scales, T, H, eps,
+                               num_sms, (cudaStream_t)st);
+           },
+           py::arg("x"), py::arg("num_recv"), py::arg("send_slot"), py::arg("bias0"), py::arg("bias1"),
+           py::arg("residual"), py::arg("residual_out"), py::arg("weight"), py::arg("out"), py::arg("out_scales"),
+           py::arg("T"), py::arg("H"), py::arg("eps"), py::arg("num_sms"), py::arg("stream"));
 
   // host reference of the LogFMT-10 simulated cast: the same arithmetic the CUDA pass compiles (ep_logfmt.h), in place
   // on [rows, H] bf16 host memory

@@ -270,18 +270,14 @@ uintptr_t EpBuffer::combine_input_ptr(int num_tokens, int hidden, int topk) {
   return (uintptr_t)(base_ + ctrl_bytes_ + (size_t)num_slots_ * arena_bytes_);
 }
 
-void EpBuffer::combine(uintptr_t x, int num_recv, uintptr_t topk_w, uintptr_t send_slot, uintptr_t bias0,
-                       uintptr_t bias1, uintptr_t out, uintptr_t out_topk_w, int T, int H, int K, int num_sms,
-                       cudaStream_t st) {
-  UB_CHECK(H > 0 && H % 8 == 0, "combine: hidden (%d) must be a multiple of 8", H);
-  UB_CHECK(K >= 0 && K <= kEpMaxTopk, "combine: bad num_topk %d", K);
-  UB_CHECK(send_slot != 0 && out != 0, "combine: handle/out missing");
-  DevGuard g(comm_->device());
+char* EpBuffer::stage_combine(const char* what, uintptr_t x, int num_recv, int H, int K, cudaStream_t st,
+                              EpCombineArgs& a) {
+  UB_CHECK(H > 0 && H % 8 == 0, "%s: hidden (%d) must be a multiple of 8", what, H);
+  UB_CHECK(K >= 0 && K <= kEpMaxTopk, "%s: bad num_topk %d", what, K);
   const int cap = combine_capacity_for(H, K);
-  UB_CHECK(num_recv <= cap, "combine: %d tokens exceed the arena capacity %d", num_recv, cap);
+  UB_CHECK(num_recv <= cap, "%s: %d tokens exceed the arena capacity %d", what, num_recv, cap);
   char* arena = base_ + ctrl_bytes_ + (size_t)num_slots_ * arena_bytes_;
   const size_t xbytes = (size_t)num_recv * H * 2;
-  EpCombineArgs a;
   memset(&a, 0, sizeof(a));
   if (x != (uintptr_t)arena && xbytes) {
     if (comm_->in_heap((void*)x, xbytes)) {
@@ -295,8 +291,18 @@ void EpBuffer::combine(uintptr_t x, int num_recv, uintptr_t topk_w, uintptr_t se
     a.x_off = comm_->heap_offset(arena);
   }
   a.topk_w_off = kNoOff;
+  return arena;
+}
+
+void EpBuffer::combine(uintptr_t x, int num_recv, uintptr_t topk_w, uintptr_t send_slot, uintptr_t bias0,
+                       uintptr_t bias1, uintptr_t out, uintptr_t out_topk_w, int T, int H, int K, int num_sms,
+                       cudaStream_t st) {
+  UB_CHECK(send_slot != 0 && out != 0, "combine: handle/out missing");
+  DevGuard g(comm_->device());
+  EpCombineArgs a;
+  char* arena = stage_combine("combine", x, num_recv, H, K, st, a);
   if (topk_w && out_topk_w && K > 0) {
-    char* wdst = arena + align_up((size_t)cap * H * 2, 256);
+    char* wdst = arena + align_up((size_t)combine_capacity_for(H, K) * H * 2, 256);
     UB_CUDA(cudaMemcpyAsync(wdst, (void*)topk_w, (size_t)num_recv * K * 4, cudaMemcpyDeviceToDevice, st));
     a.topk_w_off = comm_->heap_offset(wdst);
   }
@@ -314,6 +320,42 @@ void EpBuffer::combine(uintptr_t x, int num_recv, uintptr_t topk_w, uintptr_t se
   last_comb_impl_ = tma ? EP_IMPL_TMA : EP_IMPL_REG;
   cudaError_t e = tma ? launch_ep_combine_tma(comm_->dev(), a, grid, st) : launch_ep_combine(comm_->dev(), a, grid, st);
   UB_CHECK(e == cudaSuccess, "ep combine launch failed: %s", cudaGetErrorString(e));
+  ++launches_;
+}
+
+void EpBuffer::combine_rmsnorm(uintptr_t x, int num_recv, uintptr_t send_slot, uintptr_t bias0, uintptr_t bias1,
+                               uintptr_t residual, uintptr_t residual_out, uintptr_t weight, uintptr_t out,
+                               uintptr_t out_scales, int T, int H, float eps, int num_sms, cudaStream_t st) {
+  UB_CHECK(T >= 0, "combine_rmsnorm: bad token count %d", T);
+  // a rank without tokens still joins the kernel's barriers; its (empty) tensors may have null pointers
+  UB_CHECK(T == 0 || (send_slot != 0 && residual != 0 && residual_out != 0 && weight != 0 && out != 0),
+           "combine_rmsnorm: handle, residual, residual_out, weight or out missing");
+  UB_CHECK(H >= 8 && (uint32_t)H <= kRmsMaxH, "combine_rmsnorm: hidden size %d must be a multiple of 8 in [8, %u]", H,
+           kRmsMaxH);
+  UB_CHECK(!out_scales || H % 128 == 0, "combine_rmsnorm: fp8 output needs hidden size %% 128 == 0 (got %d)", H);
+  UB_CHECK(((bias0 | bias1 | residual | residual_out | weight | out) & 15) == 0,
+           "combine_rmsnorm: bias, residual, residual_out, weight and out must be 16-byte aligned");
+  DevGuard g(comm_->device());
+  EpCombineArgs a;
+  stage_combine("combine_rmsnorm", x, num_recv, H, 0, st, a);
+  a.send_slot = (const int32_t*)send_slot;
+  a.bias0 = (const void*)bias0;
+  a.bias1 = (const void*)bias1;
+  a.T = T;
+  a.H = H;
+  RmsNormArgs r;
+  memset(&r, 0, sizeof(r));
+  r.residual = (const void*)residual;
+  r.residual_out = (void*)residual_out;
+  r.weight = (const void*)weight;
+  r.out = (void*)out;
+  r.out_scales = (float*)out_scales;
+  r.T = (uint32_t)T;
+  r.H = (uint32_t)H;
+  r.eps = eps;
+  const int grid = std::max(1, std::min(num_sms, kEpMaxBlocks));
+  cudaError_t e = launch_ep_combine_rmsnorm(comm_->dev(), a, r, out_scales != 0, grid, st);
+  UB_CHECK(e == cudaSuccess, "ep combine_rmsnorm launch failed: %s", cudaGetErrorString(e));
   ++launches_;
 }
 

@@ -82,9 +82,18 @@ class EpBuffer {
   uintptr_t combine_input_ptr(int num_tokens, int hidden, int topk);
   void combine(uintptr_t x, int num_recv, uintptr_t topk_w, uintptr_t send_slot, uintptr_t bias0, uintptr_t bias1,
                uintptr_t out, uintptr_t out_topk_w, int T, int H, int K, int num_sms, cudaStream_t st);
+  // combine without storing the combined rows: residual_out = combined + residual (may be residual itself) and
+  // out = rmsnorm(residual_out) * weight, all [T, H] bf16; out is e4m3 with [T, H / 128] scales when out_scales != 0.
+  // H % 8 == 0 and H <= kRmsMaxH (H % 128 == 0 for e4m3).  One kernel launch (after the copy-in of a non-symmetric x).
+  void combine_rmsnorm(uintptr_t x, int num_recv, uintptr_t send_slot, uintptr_t bias0, uintptr_t bias1,
+                       uintptr_t residual, uintptr_t residual_out, uintptr_t weight, uintptr_t out,
+                       uintptr_t out_scales, int T, int H, float eps, int num_sms, cudaStream_t st);
 
  private:
   EpArena carve(int slot, int H, int mode, int K) const;
+  // checks of combine / combine_rmsnorm; zeroes `a` and sets a.x_off to the expert outputs every rank reads (x itself
+  // when it is the combine arena or symmetric, else a copy in the arena).  Returns the combine arena.
+  char* stage_combine(const char* what, uintptr_t x, int num_recv, int H, int K, cudaStream_t st, EpCombineArgs& a);
   std::shared_ptr<Comm> comm_;
   char* base_ = nullptr;      // local VA of the EP block
   uint64_t base_off_ = 0;     // its heap offset
@@ -119,6 +128,10 @@ class EpBuffer {
 cudaError_t launch_ep_layout(const EpLayoutArgs& a, cudaStream_t st);
 cudaError_t launch_ep_dispatch(const DevComm& c, const EpDispatchArgs& a, int grid, cudaStream_t st);
 cudaError_t launch_ep_combine(const DevComm& c, const EpCombineArgs& a, int grid, cudaStream_t st);
+// combine + residual add + RMSNorm [+ e4m3 cast] (ep_combine_rmsnorm.cu): a = combine arguments (a.out unused),
+// r = the epilogue's (r.x unused, r.T = a.T, r.H = a.H).  Block size kRmsThreads.
+cudaError_t launch_ep_combine_rmsnorm(const DevComm& c, const EpCombineArgs& a, const RmsNormArgs& r, bool fp8,
+                                      int grid, cudaStream_t st);
 // TMA-pipelined implementations (ep_tma_kernels.cu)
 bool ep_dispatch_tma_supported(const EpDispatchArgs& a);
 bool ep_combine_tma_supported(const EpCombineArgs& a);

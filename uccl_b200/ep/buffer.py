@@ -21,8 +21,54 @@ from typing import List, Optional, Tuple, Union
 import torch
 
 from .. import _native
-from ..parallel.comm import Communicator
+from ..parallel.comm import Communicator, _overlaps
 from .utils import EpHandle, EventHandle, EventOverlap
+
+RMS_MAX_HIDDEN = 16384  # kRmsMaxH: one 512-thread block holds a row in registers
+
+
+def _combine_rmsnorm_args(x, T, residual, weight, bias, residual_out, out, quant, device):
+    """Checks of ``combine_rmsnorm`` shared by the CUDA and the host backend.  Returns
+    ``(b0, b1, residual_out, out, scales)`` with the defaults filled in (``scales`` is None without fp8)."""
+    if x.dtype != torch.bfloat16 or x.dim() != 2 or not x.is_contiguous():
+        raise ValueError("uccl_b200.ep: combine_rmsnorm x must be contiguous bf16 [num_recv, hidden]")
+    H = x.size(1)
+    for t, name in ((residual, "residual"), (weight, "weight")):
+        if t.dtype != torch.bfloat16 or not t.is_contiguous():
+            raise ValueError(f"uccl_b200.ep: combine_rmsnorm {name} must be contiguous bf16")
+    if residual.shape != (T, H) or weight.shape != (H,):
+        raise ValueError(f"uccl_b200.ep: combine_rmsnorm needs residual [{T}, {H}] and weight [{H}] "
+                         f"(got {tuple(residual.shape)} and {tuple(weight.shape)})")
+    if H % 8 or not 8 <= H <= RMS_MAX_HIDDEN:
+        raise ValueError(f"uccl_b200.ep: combine_rmsnorm hidden size {H} must be a multiple of 8 in [8, {RMS_MAX_HIDDEN}]")
+    if quant not in (None, "fp8"):
+        raise ValueError(f"uccl_b200.ep: unsupported quant {quant!r} (None or 'fp8')")
+    fp8 = quant == "fp8"
+    if fp8 and H % 128:
+        raise ValueError(f"uccl_b200.ep: combine_rmsnorm fp8 output needs hidden size % 128 == 0 (got {H})")
+    b0, b1 = bias if isinstance(bias, tuple) else (bias, None)
+    biases = [b for b in (b0, b1) if b is not None]
+    for b in biases:
+        if b.dtype != torch.bfloat16 or b.shape != (T, H) or not b.is_contiguous():
+            raise ValueError(f"uccl_b200.ep: combine_rmsnorm bias must be contiguous bf16 [{T}, {H}]")
+    if residual_out is None:
+        residual_out = residual
+    if residual_out.dtype != torch.bfloat16 or residual_out.shape != (T, H) or not residual_out.is_contiguous():
+        raise ValueError(f"uccl_b200.ep: combine_rmsnorm residual_out must be contiguous bf16 [{T}, {H}]")
+    out_dtype = torch.float8_e4m3fn if fp8 else torch.bfloat16
+    if out is None:
+        out = torch.empty((T, H), dtype=out_dtype, device=device)
+    if out.dtype != out_dtype or out.shape != (T, H) or not out.is_contiguous():
+        raise ValueError(f"uccl_b200.ep: combine_rmsnorm out must be contiguous {out_dtype} [{T}, {H}]")
+    # peers read x while the kernel runs, and a row's residual and bias are read before its outputs are stored
+    if any(_overlaps(out, t) for t in [x, residual, residual_out] + biases):
+        raise ValueError("uccl_b200.ep: combine_rmsnorm out must not overlap x, residual, residual_out or bias")
+    if any(_overlaps(residual_out, t) for t in [x] + biases) or (
+            residual_out.data_ptr() != residual.data_ptr() and _overlaps(residual_out, residual)):
+        raise ValueError("uccl_b200.ep: combine_rmsnorm residual_out must not overlap x, bias or residual "
+                         "(it may be residual itself)")
+    scales = torch.empty((T, H // 128), dtype=torch.float32, device=device) if fp8 else None
+    return b0, b1, residual_out, out, scales
 
 
 class Config:
@@ -442,6 +488,40 @@ class Buffer:
                                  self.comm_stream.cuda_stream)
         ev = self._exit(compute, async_finish, (x, topk_weights, b0, b1, out, out_w, send_slot))
         return out, out_w, ev
+
+    def combine_rmsnorm(self, x: torch.Tensor, handle: Tuple, residual: torch.Tensor, weight: torch.Tensor,
+                        eps: float = 1e-6, *, bias: Union[torch.Tensor, Tuple[torch.Tensor, torch.Tensor], None] = None,
+                        residual_out: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+                        quant: Optional[str] = None, config: Optional[Config] = None,
+                        previous_event: Optional[EventOverlap] = None, async_finish: bool = False,
+                        allocate_on_comm_stream: bool = False):
+        """The tail of an MoE layer in one kernel: :meth:`combine`, the residual add and RMSNorm.
+
+        ``combined = combine(x, handle, bias=bias)`` (bitwise what :meth:`combine` returns) is not stored anywhere;
+        ``residual_out = bf16(combined + residual)``, written over ``residual`` unless given, and
+        ``out = rmsnorm(residual_out, eps) * weight``.  ``residual``, ``residual_out`` and ``out`` are this rank's
+        ``[T, H]`` tokens (``T = handle.send_slot.size(0)``), ``weight`` is ``[H]``, all bf16; ``H % 8 == 0`` and
+        ``H <= 16384``.  With ``quant="fp8"`` (``H % 128 == 0``) ``out`` is ``(e4m3 [T, H], fp32 scales [T, H/128])``,
+        bit-identical to ``per_token_cast_to_fp8`` of the bf16 ``out``: the input format of :meth:`dispatch`.
+        Returns ``(out, event)``.  Streams, events and ``config.num_sms`` behave as in :meth:`combine`, so the call
+        can be captured in a CUDA graph."""
+        config = config or self.get_combine_config(self.group_size)
+        send_slot, num_recv = handle.send_slot, handle.num_recv
+        T = send_slot.size(0)
+        b0, b1, residual_out, out, scales = _combine_rmsnorm_args(x, T, residual, weight, bias, residual_out, out,
+                                                                  quant, self.device)
+        if x.size(0) < num_recv:
+            raise ValueError(f"uccl_b200.ep: combine_rmsnorm x has {x.size(0)} rows, the handle {num_recv}")
+        H = x.size(1)
+        compute = self._enter(previous_event, allocate_on_comm_stream)
+        with torch.cuda.stream(self.comm_stream):
+            self.runtime.combine_rmsnorm(x.data_ptr(), x.size(0), send_slot.data_ptr(),
+                                         b0.data_ptr() if b0 is not None else 0, b1.data_ptr() if b1 is not None else 0,
+                                         residual.data_ptr(), residual_out.data_ptr(), weight.data_ptr(), out.data_ptr(),
+                                         scales.data_ptr() if scales is not None else 0, T, H, float(eps),
+                                         self._sms(config), self.comm_stream.cuda_stream)
+        ev = self._exit(compute, async_finish, (x, b0, b1, residual, residual_out, weight, out, scales, send_slot))
+        return ((out, scales) if scales is not None else out), ev
 
     # ------------------------------------------------------------------ internode entry points
     # The reference routes to RDMA+NVLink two-hop kernels when the group spans several nodes

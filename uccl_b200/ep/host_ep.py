@@ -15,7 +15,8 @@ from typing import List, Optional, Tuple, Union
 
 import torch
 
-from ..parallel.comm import Communicator
+from ..parallel.comm import Communicator, dtype_code
+from .buffer import _combine_rmsnorm_args
 from .utils import EpHandle, EventOverlap, per_token_cast_to_fp8
 
 
@@ -298,6 +299,31 @@ class HostBuffer:
             out_w = torch.zeros(T, topk_weights.size(1), dtype=torch.float32)
             out_w.index_add_(0, order, wr)
         return out.to(torch.bfloat16), out_w, EventOverlap()
+
+    def combine_rmsnorm(self, x: torch.Tensor, handle: Tuple, residual: torch.Tensor, weight: torch.Tensor,
+                        eps: float = 1e-6, *, bias=None, residual_out: Optional[torch.Tensor] = None,
+                        out: Optional[torch.Tensor] = None, quant: Optional[str] = None, config=None,
+                        previous_event=None, async_finish: bool = False, allocate_on_comm_stream: bool = False):
+        """:meth:`combine`, then the C++ epilogue of the fused layer tails (the one behind
+        ``Communicator.all_reduce_rmsnorm`` on the host backend).  Same contract as the CUDA ``combine_rmsnorm``."""
+        from .. import _native
+
+        T = handle.send_slot.size(0)
+        _, _, residual_out, out, scales = _combine_rmsnorm_args(x, T, residual, weight, bias, residual_out, out, quant,
+                                                                residual.device)
+        combined = self.combine(x, handle, bias=bias)[0].cpu()
+        # the epilogue runs on host memory; device tensors (the portable multi-box path) hop and are written back
+        res = residual.cpu()
+        ro = res if residual_out is residual else residual_out.cpu()
+        o, sc = out.cpu(), scales.cpu() if scales is not None else None
+        w = weight.cpu()
+        _native.C().host_add_rmsnorm(combined.data_ptr(), res.data_ptr(), ro.data_ptr(), w.data_ptr(), o.data_ptr(),
+                                     sc.data_ptr() if sc is not None else 0, T, x.size(1), dtype_code(torch.bfloat16),
+                                     float(eps))
+        for dst, src in ((residual_out, ro), (out, o), (scales, sc)):
+            if dst is not None and dst is not src:
+                dst.copy_(src)
+        return ((out, scales) if scales is not None else out), EventOverlap()
 
     internode_dispatch = dispatch
     internode_combine = combine
