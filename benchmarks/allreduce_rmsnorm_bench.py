@@ -30,6 +30,15 @@ every SM:
 Fused and unfused outputs are checked bitwise equal first.  The arms' graphs are replayed alternately --rounds times;
 each row reports the median, min and max per call, the bytes moved (from shapes) and the achieved rate next to the
 3.35 TB/s data sheet.  It runs on one GPU without torchrun (no NVLink traffic, HBM-bound) and under torchrun for n >= 2.
+
+--mode ll times the tail of a decode MoE layer, ep.Buffer.low_latency_combine_rmsnorm, after a bf16 low_latency_dispatch
+(top-8 of 256 experts, --tokens per rank, default 1,8,32,128, num_max_dispatch_tokens_per_rank 128, H = 7168) with a
+shared-expert output, bf16 and fp8 out:
+  fused    Buffer.low_latency_combine_rmsnorm (one kernel)
+  unfused  Buffer.low_latency_combine, + shared, then add_rmsnorm_kernel (all_reduce_rmsnorm of a one-rank communicator)
+  torch    Buffer.low_latency_combine, + shared + residual, torch.nn.functional.rms_norm [, per_token_cast_to_fp8]
+Fused and unfused outputs are checked bitwise equal first; the graphs are replayed alternately as in --mode ep.  It runs
+on one GPU without torchrun and under torchrun for n >= 2.
 """
 import argparse
 import json
@@ -175,6 +184,116 @@ def run_ep(a, rank, n, dev, dist, info):
     return rows
 
 
+def ll_fused_bytes(T, routed_rows, H, fp8):
+    """low_latency_combine_rmsnorm: read the routed expert rows, residual, shared and weight; write residual_out and
+    out (+ scales)."""
+    out = T * H + T * (H // 128) * 4 if fp8 else T * H * 2
+    return routed_rows * H * 2 + 2 * T * H * 2 + H * 2 + T * H * 2 + out
+
+
+def ll_unfused_bytes(T, routed_rows, H, fp8):
+    """low_latency_combine (read the routed rows, write [T, H]), + shared (read 2, write 1), then the epilogue."""
+    return routed_rows * H * 2 + T * H * 2 + 3 * T * H * 2 + epilogue_bytes(T, H, fp8)
+
+
+def run_ll(a, rank, n, dev, dist, info):
+    """--mode ll: see the module docstring."""
+    from uccl_b200.ep import Buffer
+
+    H, K, E, M = [int(v) for v in a.hidden.split(",")][0], 8, 256, 128
+    tokens = [int(v) for v in a.tokens.split(",")]
+    if max(tokens) > M:
+        raise SystemExit(f"--mode ll: --tokens must be <= num_max_dispatch_tokens_per_rank {M}")
+    ll = Buffer.get_low_latency_rdma_size_hint(M, H, n, E)
+    if dist is not None:
+        comm = Communicator.from_torch_dist(None, heap_bytes=ll + (256 << 20), stage_bytes=16 << 20)
+    else:
+        comm = Communicator.local_world(1, devices=[dev.index], heap_bytes=ll + (256 << 20), stage_bytes=16 << 20)[0]
+    buf = Buffer(comm=comm, num_nvl_bytes=1 << 20, num_rdma_bytes=ll, low_latency_mode=True)
+    one = Communicator.local_world(1, devices=[dev.index], heap_bytes=256 << 20, stage_bytes=8 << 20)[0]
+    g = torch.Generator(device="cpu").manual_seed(rank)
+    w = (torch.rand(H, generator=g) + 0.5).to(torch.bfloat16).to(dev)
+    rows = []
+
+    def graph_of(fn):
+        for _ in range(a.warmup):
+            fn()
+        torch.cuda.synchronize()
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            for _ in range(a.iters):
+                fn()
+        graph.replay()
+        torch.cuda.synchronize()
+        return graph
+
+    def replay_us(graph):
+        if dist is not None:
+            dist.barrier()
+        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        s.record()
+        graph.replay()
+        e.record()
+        torch.cuda.synchronize()
+        return mx(s.elapsed_time(e) / a.iters * 1e3, dist, dev)
+
+    for T in tokens:
+        x = torch.randn(T, H, generator=g).to(torch.bfloat16).to(dev)
+        idx = torch.rand(T, E, generator=g).topk(K, dim=1).indices.to(torch.int64).to(dev)
+        tw = torch.rand(T, K, generator=g).float().to(dev)
+        rx, _, handle, _, _ = buf.low_latency_dispatch(x, idx, M, E, use_fp8=False)
+        cb = buf.get_next_low_latency_combine_buffer(handle)
+        cb.copy_(rx)
+        res = torch.randn(T, H, generator=g).to(torch.bfloat16).to(dev)
+        shared = torch.randn(T, H, generator=g).to(torch.bfloat16).to(dev)
+        routed_rows = int((idx >= 0).sum())
+        torch.cuda.synchronize()
+        for fp8 in (False, True):
+            quant = "fp8" if fp8 else None
+            ro_f, ro_u = torch.empty_like(res), torch.empty_like(res)  # residual stays the input of every call
+
+            def fused():
+                return buf.low_latency_combine_rmsnorm(cb, idx, tw, handle, res, w, a.eps, shared=shared,
+                                                       residual_out=ro_f, quant=quant)[0]
+
+            def unfused():
+                c = buf.low_latency_combine(cb, idx, tw, handle)[0]
+                return one.all_reduce_rmsnorm(c + shared, res, w, a.eps, residual_out=ro_u, quant=quant)
+
+            def torch_tail():
+                c = buf.low_latency_combine(cb, idx, tw, handle)[0]
+                y = F.rms_norm(c + shared + res, (H,), w, a.eps)
+                return per_token_cast_to_fp8(y) if fp8 else y
+
+            yf, yu = fused(), unfused()
+            torch.cuda.synchronize()
+            same = torch.equal(ro_f, ro_u) and all(
+                torch.equal(p.view(torch.uint8), q.view(torch.uint8))
+                for p, q in zip(yf if fp8 else (yf,), yu if fp8 else (yu,)))
+            if not same:
+                raise SystemExit(f"--mode ll: fused and unfused outputs differ (T={T}, fp8={fp8})")
+            graphs = {"fused": graph_of(fused), "unfused": graph_of(unfused), "torch": graph_of(torch_tail)}
+            times = {k: [] for k in graphs}
+            for _ in range(a.rounds):  # alternate the arms so drift and neighbours hit them alike
+                for k, gr in graphs.items():
+                    times[k].append(replay_us(gr))
+            del graphs
+            row = {"mode": "ll", "T": T, "routed_rows": routed_rows, "H": H, "topk": K, "experts": E, "M": M,
+                   "fp8": fp8, "n_gpus": n, "bitwise_fused_eq_unfused": same, **info}
+            for k, v in times.items():
+                v = sorted(v)
+                row[f"{k}_us"] = v[len(v) // 2]
+                row[f"{k}_us_min"], row[f"{k}_us_max"] = v[0], v[-1]
+            row["fused_bytes"] = ll_fused_bytes(T, routed_rows, H, fp8)
+            row["unfused_bytes"] = ll_unfused_bytes(T, routed_rows, H, fp8)
+            row["speedup_vs_unfused"] = row["unfused_us"] / row["fused_us"]
+            row["speedup_vs_torch"] = row["torch_us"] / row["fused_us"]
+            rows.append(row)
+            if rank == 0:
+                print(json.dumps(row), flush=True)
+    return rows
+
+
 def mx(v, dist, dev):
     if dist is None:
         return v
@@ -185,22 +304,24 @@ def mx(v, dist, dev):
 
 def main():
     p = argparse.ArgumentParser()
-    p.add_argument("--mode", choices=("tp", "sp", "ep"), default="tp",
+    p.add_argument("--mode", choices=("tp", "sp", "ep", "ll"), default="tp",
                    help="tp: all_reduce_rmsnorm at decode shapes; sp: reduce_scatter_rmsnorm at prefill shapes; "
-                        "ep: ep.Buffer.combine_rmsnorm at bench.py's MoE routing")
+                        "ep: ep.Buffer.combine_rmsnorm at bench.py's MoE routing; "
+                        "ll: ep.Buffer.low_latency_combine_rmsnorm at decode shapes")
     p.add_argument("--tokens", default=None,
-                   help="default 1,4,16,64,256 (tp), 128,512,2048,8192 (sp, global T) or 128,512,4096 (ep, per rank)")
-    p.add_argument("--hidden", default=None, help="default 4096,7168,8192 (tp, sp) or 7168 (ep, first value used)")
-    p.add_argument("--rounds", type=int, default=5, help="ep: alternating replays of each arm's graph")
+                   help="default 1,4,16,64,256 (tp), 128,512,2048,8192 (sp, global T), 128,512,4096 (ep, per rank) "
+                        "or 1,8,32,128 (ll, per rank)")
+    p.add_argument("--hidden", default=None, help="default 4096,7168,8192 (tp, sp) or 7168 (ep, ll: first value used)")
+    p.add_argument("--rounds", type=int, default=5, help="ep, ll: alternating replays of each arm's graph")
     p.add_argument("--iters", type=int, default=200)
     p.add_argument("--warmup", type=int, default=20)
     p.add_argument("--eps", type=float, default=1e-6)
     p.add_argument("--out", default=None)
     a = p.parse_args()
     if a.tokens is None:
-        a.tokens = {"sp": "128,512,2048,8192", "ep": "128,512,4096"}.get(a.mode, "1,4,16,64,256")
+        a.tokens = {"sp": "128,512,2048,8192", "ep": "128,512,4096", "ll": "1,8,32,128"}.get(a.mode, "1,4,16,64,256")
     if a.hidden is None:
-        a.hidden = "7168" if a.mode == "ep" else "4096,7168,8192"
+        a.hidden = "7168" if a.mode in ("ep", "ll") else "4096,7168,8192"
     if a.mode == "sp" and int(os.environ.get("WORLD_SIZE", "1")) < 2:
         sys.exit("--mode sp needs torchrun with at least 2 ranks: on one GPU there is no reduce-scatter to time")
 
@@ -217,14 +338,14 @@ def main():
         torch.cuda.set_device(0)
         dev = torch.device("cuda", 0)
     info = card()
-    if a.mode == "ep":
-        rows = run_ep(a, rank, n, dev, dist, info)
+    if a.mode in ("ep", "ll"):
+        rows = (run_ep if a.mode == "ep" else run_ll)(a, rank, n, dev, dist, info)
         if rank == 0:
-            print(json.dumps({"mode": "ep", "n_gpus": n, **info, "shapes": len(rows)}), flush=True)
+            print(json.dumps({"mode": a.mode, "n_gpus": n, **info, "shapes": len(rows)}), flush=True)
             if a.out:
                 with open(a.out, "w") as f:
-                    json.dump({"mode": "ep", "n_gpus": n, "dtype": "bf16", "iters": a.iters, "rounds": a.rounds, **info,
-                               "rows": rows}, f, indent=1)
+                    json.dump({"mode": a.mode, "n_gpus": n, "dtype": "bf16", "iters": a.iters, "rounds": a.rounds,
+                               **info, "rows": rows}, f, indent=1)
         if dist is not None:
             dist.barrier()
             dist.destroy_process_group()

@@ -138,6 +138,13 @@ cudaError_t preload_all_kernels() {
     EpLLCombineArgs lc;
     memset(&lc, 0, sizeof(lc));
     ok(launch_ep_ll_combine(c, lc, 1, 0));
+    RmsNormArgs lr;
+    memset(&lr, 0, sizeof(lr));
+    int dummy_shared = 0;
+    for (bool fp8 : {false, true}) {
+      ok(launch_ep_ll_combine_rmsnorm(c, lc, nullptr, lr, fp8, 1, 0));
+      ok(launch_ep_ll_combine_rmsnorm(c, lc, &dummy_shared, lr, fp8, 1, 0));
+    }
     EpLLPackArgs lp;
     memset(&lp, 0, sizeof(lp));
     ok(launch_ep_ll_pack(lp, 0));

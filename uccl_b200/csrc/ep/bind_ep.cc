@@ -103,6 +103,19 @@ void bind_ep(py::module_& m) {
            py::arg("T"), py::arg("H"), py::arg("K"), py::arg("E"), py::arg("M"), py::arg("num_sms"), py::arg("stream"),
            py::arg("phase") = (int)EP_LL_FULL, py::arg("layout_range") = 0, py::arg("wait_stats") = 0,
            py::arg("use_logfmt") = false)
+      .def("ll_combine_rmsnorm",
+           [](EpBuffer& b, uintptr_t x, int idx, uintptr_t tw, uintptr_t sp, uintptr_t shared, uintptr_t residual,
+              uintptr_t residual_out, uintptr_t weight, uintptr_t out, uintptr_t out_scales, int T, int H, int K, int E,
+              int M, float eps, int num_sms, uintptr_t st, int phase, uintptr_t layout_range, uintptr_t wait_stats,
+              bool use_logfmt) {
+             b.ll_combine_rmsnorm(x, idx, tw, sp, shared, residual, residual_out, weight, out, out_scales, T, H, K, E,
+                                  M, eps, num_sms, (cudaStream_t)st, phase, layout_range, wait_stats, use_logfmt);
+           },
+           py::arg("x"), py::arg("buffer_idx"), py::arg("topk_weights"), py::arg("send_pos"), py::arg("shared"),
+           py::arg("residual"), py::arg("residual_out"), py::arg("weight"), py::arg("out"), py::arg("out_scales"),
+           py::arg("T"), py::arg("H"), py::arg("K"), py::arg("E"), py::arg("M"), py::arg("eps"), py::arg("num_sms"),
+           py::arg("stream"), py::arg("phase") = (int)EP_LL_FULL, py::arg("layout_range") = 0,
+           py::arg("wait_stats") = 0, py::arg("use_logfmt") = false)
       .def("combine_input_ptr", &EpBuffer::combine_input_ptr)
       .def("combine", [](EpBuffer& b, uintptr_t x, int num_recv, uintptr_t tw, uintptr_t ss, uintptr_t b0,
                          uintptr_t b1, uintptr_t out, uintptr_t otw, int T, int H, int K, int num_sms, uintptr_t st) {

@@ -488,16 +488,15 @@ uintptr_t EpBuffer::ll_combine_buffer(int buffer_idx, int H, int E, int M) const
   return (uintptr_t)(comm_->fabric().local() + l.comb_x_off);
 }
 
-void EpBuffer::ll_combine(uintptr_t x, int buffer_idx, uintptr_t topk_w, uintptr_t send_pos, uintptr_t out, int T,
-                          int H, int K, int E, int M, int num_sms, cudaStream_t st, int phase, uintptr_t layout_range,
-                          uintptr_t wait_stats, bool use_logfmt) {
+uint64_t EpBuffer::ll_stage_combine(const char* what, uintptr_t x, int buffer_idx, int H, int E, int M,
+                                    cudaStream_t st, int phase, uintptr_t layout_range, bool use_logfmt) {
   const int R = nranks();
-  UB_CHECK(phase >= EP_LL_FULL && phase <= EP_LL_RECV, "ll_combine: bad phase %d", phase);
-  DevGuard g(comm_->device());
+  UB_CHECK(phase >= EP_LL_FULL && phase <= EP_LL_RECV, "%s: bad phase %d", what, phase);
   LLLayout l = ll_layout(buffer_idx, H, E, M);
   char* arena = comm_->fabric().local() + l.comb_x_off;
   if (use_logfmt && phase != EP_LL_RECV)
-    UB_CHECK(layout_range != 0 && H % 128 == 0, "ll_combine: use_logfmt needs layout_range and hidden %% 128 == 0 (H = %d)", H);
+    UB_CHECK(layout_range != 0 && H % 128 == 0, "%s: use_logfmt needs layout_range and hidden %% 128 == 0 (H = %d)",
+             what, H);
   if ((x != (uintptr_t)arena || use_logfmt) && phase != EP_LL_RECV) {
     // expert outputs that do not live in the symmetric buffer: bring them in, occupied rows only; with use_logfmt
     // the same pass applies the reference's simulated LogFMT-10 cast (in place when x already is the buffer)
@@ -519,9 +518,16 @@ void EpBuffer::ll_combine(uintptr_t x, int buffer_idx, uintptr_t topk_w, uintptr
       UB_CUDA(cudaMemcpyAsync(arena, (void*)x, bytes, cudaMemcpyDeviceToDevice, st));
     }
   }
+  return l.comb_x_off;
+}
+
+void EpBuffer::ll_combine(uintptr_t x, int buffer_idx, uintptr_t topk_w, uintptr_t send_pos, uintptr_t out, int T,
+                          int H, int K, int E, int M, int num_sms, cudaStream_t st, int phase, uintptr_t layout_range,
+                          uintptr_t wait_stats, bool use_logfmt) {
+  DevGuard g(comm_->device());
   EpLLCombineArgs a;
   memset(&a, 0, sizeof(a));
-  a.x_off = l.comb_x_off;
+  a.x_off = ll_stage_combine("ll_combine", x, buffer_idx, H, E, M, st, phase, layout_range, use_logfmt);
   a.send_pos = (const int64_t*)send_pos;
   a.topk_weights = (const float*)topk_w;
   a.out = (void*)out;
@@ -533,6 +539,53 @@ void EpBuffer::ll_combine(uintptr_t x, int buffer_idx, uintptr_t topk_w, uintptr
   int grid = std::max(1, std::min(num_sms, kEpMaxBlocks));
   cudaError_t e = launch_ep_ll_combine(comm_->dev(), a, grid, st);
   UB_CHECK(e == cudaSuccess, "ep ll_combine launch failed: %s", cudaGetErrorString(e));
+  ++launches_;
+}
+
+void EpBuffer::ll_combine_rmsnorm(uintptr_t x, int buffer_idx, uintptr_t topk_w, uintptr_t send_pos, uintptr_t shared,
+                                  uintptr_t residual, uintptr_t residual_out, uintptr_t weight, uintptr_t out,
+                                  uintptr_t out_scales, int T, int H, int K, int E, int M, float eps, int num_sms,
+                                  cudaStream_t st, int phase, uintptr_t layout_range, uintptr_t wait_stats,
+                                  bool use_logfmt) {
+  UB_CHECK(T >= 0, "ll_combine_rmsnorm: bad token count %d", T);
+  UB_CHECK(K > 0 && K <= 32, "ll_combine_rmsnorm: bad num_topk %d", K);
+  UB_CHECK(H > 0 && H % 128 == 0 && H <= 8192, "ll_combine_rmsnorm: hidden must be a multiple of 128 and <= 8192 (got %d)",
+           H);
+  // a rank without tokens still joins the kernel's barriers; its (empty) tensors may have null pointers
+  UB_CHECK(T == 0 || (topk_w != 0 && send_pos != 0 && residual != 0 && residual_out != 0 && weight != 0 && out != 0),
+           "ll_combine_rmsnorm: topk_weights, send_pos, residual, residual_out, weight or out missing");
+  UB_CHECK(((shared | residual | residual_out | weight | out | out_scales) & 15) == 0,
+           "ll_combine_rmsnorm: shared, residual, residual_out, weight, out and scales must be 16-byte aligned");
+  DevGuard g(comm_->device());
+  EpLLCombineArgs a;
+  memset(&a, 0, sizeof(a));
+  a.x_off = ll_stage_combine("ll_combine_rmsnorm", x, buffer_idx, H, E, M, st, phase, layout_range, use_logfmt);
+  a.send_pos = (const int64_t*)send_pos;
+  a.topk_weights = (const float*)topk_w;
+  a.T = T;
+  a.H = H;
+  a.K = K;
+  a.phase = phase;
+  a.wait_stats = (long long*)wait_stats;
+  const int grid = std::max(1, std::min(num_sms, kEpMaxBlocks));
+  cudaError_t e;
+  if (phase == EP_LL_SEND) {
+    // the pull design's send half only announces that the expert outputs are in place: the plain combine's
+    e = launch_ep_ll_combine(comm_->dev(), a, grid, st);
+  } else {
+    RmsNormArgs r;
+    memset(&r, 0, sizeof(r));
+    r.residual = (const void*)residual;
+    r.residual_out = (void*)residual_out;
+    r.weight = (const void*)weight;
+    r.out = (void*)out;
+    r.out_scales = (float*)out_scales;
+    r.T = (uint32_t)T;
+    r.H = (uint32_t)H;
+    r.eps = eps;
+    e = launch_ep_ll_combine_rmsnorm(comm_->dev(), a, (const void*)shared, r, out_scales != 0, grid, st);
+  }
+  UB_CHECK(e == cudaSuccess, "ep ll_combine_rmsnorm launch failed: %s", cudaGetErrorString(e));
   ++launches_;
 }
 

@@ -77,6 +77,15 @@ class EpBuffer {
   void ll_combine(uintptr_t x, int buffer_idx, uintptr_t topk_w, uintptr_t send_pos, uintptr_t out, int T, int H, int K,
                   int E, int M, int num_sms, cudaStream_t st, int phase = EP_LL_FULL, uintptr_t layout_range = 0,
                   uintptr_t wait_stats = 0, bool use_logfmt = false);
+  // ll_combine without storing the combined rows: combined = routed [+ shared, rounded to bf16 once more],
+  // residual_out = combined + residual (may be residual itself), out = rmsnorm(residual_out) * weight, all [T, H]
+  // bf16; out is e4m3 with [T, H / 128] scales when out_scales != 0.  H % 128 == 0, H <= 8192.  EP_LL_SEND launches
+  // the plain combine's send half, EP_LL_FULL / _RECV the fused kernel.  One launch with an x that is the combine
+  // buffer and no logfmt.
+  void ll_combine_rmsnorm(uintptr_t x, int buffer_idx, uintptr_t topk_w, uintptr_t send_pos, uintptr_t shared,
+                          uintptr_t residual, uintptr_t residual_out, uintptr_t weight, uintptr_t out,
+                          uintptr_t out_scales, int T, int H, int K, int E, int M, float eps, int num_sms,
+                          cudaStream_t st, int phase, uintptr_t layout_range, uintptr_t wait_stats, bool use_logfmt);
 
   // zero-copy combine input: a [num_tokens, hidden] bf16 view of the combine arena
   uintptr_t combine_input_ptr(int num_tokens, int hidden, int topk);
@@ -117,6 +126,10 @@ class EpBuffer {
     uint64_t cnt_tab_off, recv_x_off, recv_scales_off, recv_src_off, comb_x_off;
   };
   LLLayout ll_layout(int buffer_idx, int H, int E, int M) const;
+  // checks of ll_combine / ll_combine_rmsnorm, and (except in the RECV phase) the copy-in of an x that is not the
+  // LL combine buffer buffer_idx, or its in-place LogFMT pass.  Returns the heap offset of that buffer.
+  uint64_t ll_stage_combine(const char* what, uintptr_t x, int buffer_idx, int H, int E, int M, cudaStream_t st,
+                            int phase, uintptr_t layout_range, bool use_logfmt);
   char* ll_base_ = nullptr;
   size_t ll_bytes_ = 0;
   int ll_next_ = 0;
@@ -139,6 +152,11 @@ cudaError_t launch_ep_dispatch_tma(const DevComm& c, const EpDispatchArgs& a, in
 cudaError_t launch_ep_combine_tma(const DevComm& c, const EpCombineArgs& a, int grid, cudaStream_t st);
 cudaError_t launch_ep_ll_dispatch(const DevComm& c, const EpLLDispatchArgs& a, int grid, cudaStream_t st);
 cudaError_t launch_ep_ll_combine(const DevComm& c, const EpLLCombineArgs& a, int grid, cudaStream_t st);
+// LL combine + optional shared-expert add + residual add + RMSNorm [+ e4m3 cast] (ep_ll_combine_rmsnorm.cu): a = LL
+// combine arguments (a.out unused; phase FULL or RECV), shared = optional [T, H] bf16, r = the epilogue's (r.x unused,
+// r.T = a.T, r.H = a.H <= 8192).  Block size kRmsThreads, the grid of launch_ep_ll_combine.
+cudaError_t launch_ep_ll_combine_rmsnorm(const DevComm& c, const EpLLCombineArgs& a, const void* shared,
+                                         const RmsNormArgs& r, bool fp8, int grid, cudaStream_t st);
 cudaError_t launch_ep_ll_pack(const EpLLPackArgs& a, cudaStream_t st);
 constexpr int kEpLLMaxBlocks = 128;  // one CTA per token of a decode batch
 

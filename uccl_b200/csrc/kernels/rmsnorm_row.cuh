@@ -2,6 +2,8 @@
 // row held in registers by a block of kRmsThreads threads.  Shared by allreduce_rmsnorm.cu (TP / SP tails and the
 // local add_rmsnorm_kernel) and ep/ep_combine_rmsnorm.cu (EP combine tail).  Every caller uses the identical
 // thread -> element mapping (unit k * kRmsThreads + threadIdx.x of the row), so their results are bitwise equal.
+// U (default kRmsUnits) is the number of units a thread holds: a caller whose rows are shorter (the low-latency EP
+// combine, H <= 8192, needs 2) passes fewer and saves the registers of the units it can never have.
 #pragma once
 #include "fp8_quant.cuh"
 #include "reduce.cuh"
@@ -16,12 +18,12 @@ __device__ __forceinline__ float round_to(float v) {
 
 // Load half: the thread's units of the residual row.  Callers that also load the values to normalise issue both
 // before the first use, so a row costs one memory round trip instead of two.
-template <typename T>
-__device__ __forceinline__ void rmsnorm_load_residual(uint4 (&res)[kRmsUnits], uint64_t row, const RmsNormArgs& r) {
+template <typename T, int U = kRmsUnits>
+__device__ __forceinline__ void rmsnorm_load_residual(uint4 (&res)[U], uint64_t row, const RmsNormArgs& r) {
   const uint32_t upr = r.H / 8;  // 16-byte units per row
   const uint64_t base = row * upr;
 #pragma unroll
-  for (int k = 0; k < kRmsUnits; ++k) {
+  for (int k = 0; k < U; ++k) {
     const uint32_t u = k * kRmsThreads + threadIdx.x;
     if (u < upr) res[k] = ld_v4(static_cast<const char*>(r.residual) + (base + u) * 16);
   }
@@ -31,16 +33,16 @@ __device__ __forceinline__ void rmsnorm_load_residual(uint4 (&res)[kRmsUnits], u
 // row, res[k] the same units of the residual (rmsnorm_load_residual).  The whole residual row is loaded before
 // anything is stored, and every thread only stores the units it loaded, so residual_out may alias residual.  All
 // kRmsThreads threads of the block must call it.
-template <typename T, bool FP8>
-__device__ __forceinline__ void rmsnorm_row_loaded(float (&v)[kRmsUnits][8], const uint4 (&res)[kRmsUnits],
-                                                   uint64_t row, const RmsNormArgs& r, float* s_warp) {
+template <typename T, bool FP8, int U = kRmsUnits>
+__device__ __forceinline__ void rmsnorm_row_loaded(float (&v)[U][8], const uint4 (&res)[U], uint64_t row,
+                                                   const RmsNormArgs& r, float* s_warp) {
   const int tid = threadIdx.x;
   const uint32_t upr = r.H / 8;
   const uint64_t base = row * upr;
   // residual add, rounded to T; sum of squares of the rounded values in a fixed order
   float ss = 0.f;
 #pragma unroll
-  for (int k = 0; k < kRmsUnits; ++k) {
+  for (int k = 0; k < U; ++k) {
     const uint32_t u = k * kRmsThreads + tid;
     if (u < upr) {
       Vec16<T, kSum> rv;
@@ -66,7 +68,7 @@ __device__ __forceinline__ void rmsnorm_row_loaded(float (&v)[kRmsUnits][8], con
   const float inv = rsqrtf(__fdiv_rn(tot, (float)r.H) + r.eps);
 
 #pragma unroll
-  for (int k = 0; k < kRmsUnits; ++k) {
+  for (int k = 0; k < U; ++k) {
     if (k * kRmsThreads >= (int)upr) break;  // block-uniform: the fp8 path shuffles below
     const uint32_t u = k * kRmsThreads + tid;
     const bool valid = u < upr;

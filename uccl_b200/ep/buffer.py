@@ -25,6 +25,48 @@ from ..parallel.comm import Communicator, _overlaps
 from .utils import EpHandle, EventHandle, EventOverlap
 
 RMS_MAX_HIDDEN = 16384  # kRmsMaxH: one 512-thread block holds a row in registers
+LL_MAX_HIDDEN = 8192  # limit of the low-latency kernels
+LL_MAX_TOPK = 32
+
+
+def _rmsnorm_tail_args(name, x, T, H, residual, weight, extra, extra_name, residual_out, out, quant, device):
+    """Checks shared by the fused EP tails (``combine_rmsnorm``, ``low_latency_combine_rmsnorm``) on the CUDA and the
+    host backend, once ``x`` and ``H`` are checked: ``residual`` / ``weight``, the ``[T, H]`` inputs ``extra`` that are
+    added to the combined rows (``extra_name``: bias or shared), ``quant``, ``residual_out`` and ``out``, and that no
+    output overlaps an input.  Returns ``(residual_out, out, scales)`` with the defaults filled in (``scales`` is None
+    without fp8)."""
+    for t, nm in ((residual, "residual"), (weight, "weight")):
+        if t.dtype != torch.bfloat16 or not t.is_contiguous():
+            raise ValueError(f"uccl_b200.ep: {name} {nm} must be contiguous bf16")
+    if residual.shape != (T, H) or weight.shape != (H,):
+        raise ValueError(f"uccl_b200.ep: {name} needs residual [{T}, {H}] and weight [{H}] "
+                         f"(got {tuple(residual.shape)} and {tuple(weight.shape)})")
+    if quant not in (None, "fp8"):
+        raise ValueError(f"uccl_b200.ep: unsupported quant {quant!r} (None or 'fp8')")
+    fp8 = quant == "fp8"
+    if fp8 and H % 128:
+        raise ValueError(f"uccl_b200.ep: {name} fp8 output needs hidden size % 128 == 0 (got {H})")
+    for b in extra:
+        if b.dtype != torch.bfloat16 or b.shape != (T, H) or not b.is_contiguous():
+            raise ValueError(f"uccl_b200.ep: {name} {extra_name} must be contiguous bf16 [{T}, {H}]")
+    if residual_out is None:
+        residual_out = residual
+    if residual_out.dtype != torch.bfloat16 or residual_out.shape != (T, H) or not residual_out.is_contiguous():
+        raise ValueError(f"uccl_b200.ep: {name} residual_out must be contiguous bf16 [{T}, {H}]")
+    out_dtype = torch.float8_e4m3fn if fp8 else torch.bfloat16
+    if out is None:
+        out = torch.empty((T, H), dtype=out_dtype, device=device)
+    if out.dtype != out_dtype or out.shape != (T, H) or not out.is_contiguous():
+        raise ValueError(f"uccl_b200.ep: {name} out must be contiguous {out_dtype} [{T}, {H}]")
+    # peers read x while the kernel runs, and a row's residual and extra inputs are read before its outputs are stored
+    if any(_overlaps(out, t) for t in [x, residual, residual_out] + list(extra)):
+        raise ValueError(f"uccl_b200.ep: {name} out must not overlap x, residual, residual_out or {extra_name}")
+    if any(_overlaps(residual_out, t) for t in [x] + list(extra)) or (
+            residual_out.data_ptr() != residual.data_ptr() and _overlaps(residual_out, residual)):
+        raise ValueError(f"uccl_b200.ep: {name} residual_out must not overlap x, {extra_name} or residual "
+                         "(it may be residual itself)")
+    scales = torch.empty((T, H // 128), dtype=torch.float32, device=device) if fp8 else None
+    return residual_out, out, scales
 
 
 def _combine_rmsnorm_args(x, T, residual, weight, bias, residual_out, out, quant, device):
@@ -33,42 +75,35 @@ def _combine_rmsnorm_args(x, T, residual, weight, bias, residual_out, out, quant
     if x.dtype != torch.bfloat16 or x.dim() != 2 or not x.is_contiguous():
         raise ValueError("uccl_b200.ep: combine_rmsnorm x must be contiguous bf16 [num_recv, hidden]")
     H = x.size(1)
-    for t, name in ((residual, "residual"), (weight, "weight")):
-        if t.dtype != torch.bfloat16 or not t.is_contiguous():
-            raise ValueError(f"uccl_b200.ep: combine_rmsnorm {name} must be contiguous bf16")
-    if residual.shape != (T, H) or weight.shape != (H,):
-        raise ValueError(f"uccl_b200.ep: combine_rmsnorm needs residual [{T}, {H}] and weight [{H}] "
-                         f"(got {tuple(residual.shape)} and {tuple(weight.shape)})")
     if H % 8 or not 8 <= H <= RMS_MAX_HIDDEN:
         raise ValueError(f"uccl_b200.ep: combine_rmsnorm hidden size {H} must be a multiple of 8 in [8, {RMS_MAX_HIDDEN}]")
-    if quant not in (None, "fp8"):
-        raise ValueError(f"uccl_b200.ep: unsupported quant {quant!r} (None or 'fp8')")
-    fp8 = quant == "fp8"
-    if fp8 and H % 128:
-        raise ValueError(f"uccl_b200.ep: combine_rmsnorm fp8 output needs hidden size % 128 == 0 (got {H})")
     b0, b1 = bias if isinstance(bias, tuple) else (bias, None)
     biases = [b for b in (b0, b1) if b is not None]
-    for b in biases:
-        if b.dtype != torch.bfloat16 or b.shape != (T, H) or not b.is_contiguous():
-            raise ValueError(f"uccl_b200.ep: combine_rmsnorm bias must be contiguous bf16 [{T}, {H}]")
-    if residual_out is None:
-        residual_out = residual
-    if residual_out.dtype != torch.bfloat16 or residual_out.shape != (T, H) or not residual_out.is_contiguous():
-        raise ValueError(f"uccl_b200.ep: combine_rmsnorm residual_out must be contiguous bf16 [{T}, {H}]")
-    out_dtype = torch.float8_e4m3fn if fp8 else torch.bfloat16
-    if out is None:
-        out = torch.empty((T, H), dtype=out_dtype, device=device)
-    if out.dtype != out_dtype or out.shape != (T, H) or not out.is_contiguous():
-        raise ValueError(f"uccl_b200.ep: combine_rmsnorm out must be contiguous {out_dtype} [{T}, {H}]")
-    # peers read x while the kernel runs, and a row's residual and bias are read before its outputs are stored
-    if any(_overlaps(out, t) for t in [x, residual, residual_out] + biases):
-        raise ValueError("uccl_b200.ep: combine_rmsnorm out must not overlap x, residual, residual_out or bias")
-    if any(_overlaps(residual_out, t) for t in [x] + biases) or (
-            residual_out.data_ptr() != residual.data_ptr() and _overlaps(residual_out, residual)):
-        raise ValueError("uccl_b200.ep: combine_rmsnorm residual_out must not overlap x, bias or residual "
-                         "(it may be residual itself)")
-    scales = torch.empty((T, H // 128), dtype=torch.float32, device=device) if fp8 else None
+    residual_out, out, scales = _rmsnorm_tail_args("combine_rmsnorm", x, T, H, residual, weight, biases, "bias",
+                                                   residual_out, out, quant, device)
     return b0, b1, residual_out, out, scales
+
+
+def _ll_combine_rmsnorm_args(x, topk_idx, topk_weights, R, M, H, E, residual, weight, shared, residual_out, out, quant,
+                             device):
+    """Checks of ``low_latency_combine_rmsnorm`` shared by the CUDA and the host backend (``R`` ranks; ``M``, ``H``
+    and ``E`` from the dispatch handle).  Returns ``(T, K, residual_out, out, scales)`` with the defaults filled in."""
+    name = "low_latency_combine_rmsnorm"
+    if topk_weights.dtype != torch.float32 or topk_weights.dim() != 2 or not topk_weights.is_contiguous():
+        raise ValueError(f"uccl_b200.ep: {name} topk_weights must be contiguous float32 [num_tokens, num_topk]")
+    T, K = topk_weights.shape
+    if not 0 < K <= LL_MAX_TOPK:
+        raise ValueError(f"uccl_b200.ep: {name} num_topk {K} must be in [1, {LL_MAX_TOPK}]")
+    if topk_idx.dtype != torch.int64 or topk_idx.shape != (T, K):
+        raise ValueError(f"uccl_b200.ep: {name} topk_idx must be int64 [{T}, {K}] like topk_weights")
+    if H % 128 or not 128 <= H <= LL_MAX_HIDDEN:
+        raise ValueError(f"uccl_b200.ep: {name} hidden size {H} must be a multiple of 128 in [128, {LL_MAX_HIDDEN}]")
+    if x.dtype != torch.bfloat16 or x.shape != (E // R, R * M, H) or not x.is_contiguous():
+        raise ValueError(f"uccl_b200.ep: {name} x must be contiguous bf16 [{E // R}, {R * M}, {H}] "
+                         f"(got {x.dtype} {tuple(x.shape)})")
+    extra = [shared] if shared is not None else []
+    return (T, K) + _rmsnorm_tail_args(name, x, T, H, residual, weight, extra, "shared", residual_out, out, quant,
+                                       device)
 
 
 class Config:
@@ -619,6 +654,32 @@ class Buffer:
 
     def low_latency_combine(self, x, topk_idx, topk_weights, handle, **kw):
         return self._need_ll().combine(x, topk_idx, topk_weights, handle, **kw)
+
+    def low_latency_combine_rmsnorm(self, x: torch.Tensor, topk_idx: torch.Tensor, topk_weights: torch.Tensor, handle,
+                                    residual: torch.Tensor, weight: torch.Tensor, eps: float = 1e-6, *,
+                                    shared: Optional[torch.Tensor] = None, residual_out: Optional[torch.Tensor] = None,
+                                    out: Optional[torch.Tensor] = None, quant: Optional[str] = None,
+                                    use_logfmt: bool = False, zero_copy: bool = False, async_finish: bool = False,
+                                    return_recv_hook: bool = False,
+                                    combine_wait_recv_cost_stats: Optional[torch.Tensor] = None):
+        """The tail of a decode MoE layer in one kernel: :meth:`low_latency_combine`, the shared-expert add, the residual
+        add and RMSNorm.
+
+        ``routed = low_latency_combine(x, topk_idx, topk_weights, handle, use_logfmt=...)`` (bitwise what that call
+        returns) is not stored anywhere; ``combined = routed``, or ``bf16(routed + shared)`` with a shared-expert output
+        (exactly torch's bf16 ``routed + shared``: unlike :meth:`combine_rmsnorm`'s ``bias``, which is added in fp32
+        before the single rounding, ``shared`` is added after ``routed`` is rounded, as unfused decode code does);
+        ``residual_out = bf16(combined + residual)``, written over ``residual`` unless given, and
+        ``out = rmsnorm(residual_out, eps) * weight``.  ``residual``, ``residual_out``, ``shared`` and ``out`` are this
+        rank's ``[T, H]`` tokens (``T = topk_weights.size(0)``), ``weight`` is ``[H]``, all bf16; the LL limits hold
+        (``H % 128 == 0``, ``H <= 8192``, ``K <= 32``).  With ``quant="fp8"`` ``out`` is
+        ``(e4m3 [T, H], fp32 scales [T, H/128])``, bit-identical to ``per_token_cast_to_fp8`` of the bf16 ``out``.
+        Returns ``(out, event, hook)`` like :meth:`low_latency_combine`; with ``return_recv_hook=True`` the send half
+        runs now and the fused receive half when ``hook()`` is called (or by the next low-latency call)."""
+        return self._need_ll().combine_rmsnorm(
+            x, topk_idx, topk_weights, handle, residual, weight, eps, shared=shared, residual_out=residual_out, out=out,
+            quant=quant, use_logfmt=use_logfmt, zero_copy=zero_copy, async_finish=async_finish,
+            return_recv_hook=return_recv_hook, combine_wait_recv_cost_stats=combine_wait_recv_cost_stats)
 
     def get_next_low_latency_combine_buffer(self, handle):
         return self._need_ll().next_combine_buffer(handle)

@@ -16,7 +16,7 @@ from typing import List, Optional, Tuple, Union
 import torch
 
 from ..parallel.comm import Communicator, dtype_code
-from .buffer import _combine_rmsnorm_args
+from .buffer import _combine_rmsnorm_args, _ll_combine_rmsnorm_args
 from .utils import EpHandle, EventOverlap, per_token_cast_to_fp8
 
 
@@ -95,6 +95,25 @@ def _portable(fn):
         return to_dev(res, seen[0])
 
     return wrapper
+
+
+def _host_add_rmsnorm(combined, residual, residual_out, weight, out, scales, eps):
+    """The C++ epilogue of the fused layer tails (the one behind ``Communicator.all_reduce_rmsnorm`` on the host
+    backend) on already combined [T, H] bf16 rows.  It runs on host memory; device tensors (the portable multi-box
+    path) hop and are written back."""
+    from .. import _native
+
+    T, H = combined.shape
+    combined = combined.cpu().contiguous()
+    res = residual.cpu()
+    ro = res if residual_out is residual else residual_out.cpu()
+    o, sc = out.cpu(), scales.cpu() if scales is not None else None
+    w = weight.cpu()
+    _native.C().host_add_rmsnorm(combined.data_ptr(), res.data_ptr(), ro.data_ptr(), w.data_ptr(), o.data_ptr(),
+                                 sc.data_ptr() if sc is not None else 0, T, H, dtype_code(torch.bfloat16), float(eps))
+    for dst, src in ((residual_out, ro), (out, o), (scales, sc)):
+        if dst is not None and dst is not src:
+            dst.copy_(src)
 
 
 class HostBuffer:
@@ -306,23 +325,11 @@ class HostBuffer:
                         previous_event=None, async_finish: bool = False, allocate_on_comm_stream: bool = False):
         """:meth:`combine`, then the C++ epilogue of the fused layer tails (the one behind
         ``Communicator.all_reduce_rmsnorm`` on the host backend).  Same contract as the CUDA ``combine_rmsnorm``."""
-        from .. import _native
-
         T = handle.send_slot.size(0)
         _, _, residual_out, out, scales = _combine_rmsnorm_args(x, T, residual, weight, bias, residual_out, out, quant,
                                                                 residual.device)
-        combined = self.combine(x, handle, bias=bias)[0].cpu()
-        # the epilogue runs on host memory; device tensors (the portable multi-box path) hop and are written back
-        res = residual.cpu()
-        ro = res if residual_out is residual else residual_out.cpu()
-        o, sc = out.cpu(), scales.cpu() if scales is not None else None
-        w = weight.cpu()
-        _native.C().host_add_rmsnorm(combined.data_ptr(), res.data_ptr(), ro.data_ptr(), w.data_ptr(), o.data_ptr(),
-                                     sc.data_ptr() if sc is not None else 0, T, x.size(1), dtype_code(torch.bfloat16),
-                                     float(eps))
-        for dst, src in ((residual_out, ro), (out, o), (scales, sc)):
-            if dst is not None and dst is not src:
-                dst.copy_(src)
+        combined = self.combine(x, handle, bias=bias)[0]
+        _host_add_rmsnorm(combined, residual, residual_out, weight, out, scales, eps)
         return ((out, scales) if scales is not None else out), EventOverlap()
 
     internode_dispatch = dispatch
@@ -471,3 +478,23 @@ class HostBuffer:
             res = out
         hook = (lambda: None) if return_recv_hook else None
         return res, EventOverlap(), hook
+
+    def low_latency_combine_rmsnorm(self, x: torch.Tensor, topk_idx: torch.Tensor, topk_weights: torch.Tensor, handle,
+                                    residual: torch.Tensor, weight: torch.Tensor, eps: float = 1e-6, *,
+                                    shared: Optional[torch.Tensor] = None, residual_out: Optional[torch.Tensor] = None,
+                                    out: Optional[torch.Tensor] = None, quant: Optional[str] = None,
+                                    use_logfmt: bool = False, zero_copy: bool = False, async_finish: bool = False,
+                                    return_recv_hook: bool = False, combine_wait_recv_cost_stats=None):
+        """:meth:`low_latency_combine`, torch's bf16 ``+ shared``, then the C++ epilogue of the fused layer tails (as
+        in :meth:`combine_rmsnorm`).  Same contract as the CUDA ``low_latency_combine_rmsnorm``."""
+        M, H, E = handle[2:5]
+        _, _, residual_out, out, scales = _ll_combine_rmsnorm_args(x, topk_idx, topk_weights, self.group_size, M, H, E,
+                                                                   residual, weight, shared, residual_out, out, quant,
+                                                                   residual.device)
+        combined = self.low_latency_combine(x, topk_idx, topk_weights, handle, use_logfmt=use_logfmt,
+                                            zero_copy=zero_copy)[0].cpu()
+        if shared is not None:
+            combined = combined + shared.cpu()  # bf16 + bf16, rounded once: what unfused decode code computes
+        _host_add_rmsnorm(combined, residual, residual_out, weight, out, scales, eps)
+        hook = (lambda: None) if return_recv_hook else None
+        return ((out, scales) if scales is not None else out), EventOverlap(), hook

@@ -212,3 +212,64 @@ class LowLatencyRuntime:
                                wait_stats=stats_ptr, use_logfmt=bool(use_logfmt))
         ev = EventOverlap(EventHandle(st)) if async_finish else EventOverlap()
         return out, ev, hook
+
+    def combine_rmsnorm(self, x: torch.Tensor, topk_idx: torch.Tensor, topk_weights: torch.Tensor, handle,
+                        residual: torch.Tensor, weight: torch.Tensor, eps: float = 1e-6, *,
+                        shared: Optional[torch.Tensor] = None, residual_out: Optional[torch.Tensor] = None,
+                        out: Optional[torch.Tensor] = None, quant: Optional[str] = None, use_logfmt: bool = False,
+                        zero_copy: bool = False, async_finish: bool = False, return_recv_hook: bool = False,
+                        combine_wait_recv_cost_stats: Optional[torch.Tensor] = None):
+        """``Buffer.low_latency_combine_rmsnorm``: :meth:`combine` with the shared-expert add, residual add and RMSNorm
+        fused into its receive half.  The send half (copy-in or LogFMT pass, then the announcement) is combine's."""
+        from .buffer import _ll_combine_rmsnorm_args
+
+        if use_logfmt and zero_copy:
+            raise ValueError("uccl_b200.ep: zero_copy and use_logfmt are mutually exclusive (as in the reference)")
+        assert not (async_finish and return_recv_hook), "async_finish and return_recv_hook are mutually exclusive"
+        src_info, layout_range, M, H, E, idx, send_pos = handle
+        b = self.buf
+        C = b._C
+        R = b.group_size
+        dev = b.device
+        T, K, residual_out, out, scales = _ll_combine_rmsnorm_args(
+            x, topk_idx, topk_weights, R, M, H, E, residual, weight, shared, residual_out, out, quant, dev)
+        if T > send_pos.size(0) or K != send_pos.size(1):
+            raise ValueError(f"uccl_b200.ep: low_latency_combine_rmsnorm got topk_weights [{T}, {K}] for a dispatch of "
+                             f"{tuple(send_pos.shape)}")
+        if combine_wait_recv_cost_stats is not None:
+            assert combine_wait_recv_cost_stats.dtype == torch.int64 and combine_wait_recv_cost_stats.numel() >= R
+        stats_ptr = combine_wait_recv_cost_stats.data_ptr() if combine_wait_recv_cost_stats is not None else 0
+        self._finish_pending()
+        st = torch.cuda.current_stream(dev)
+        sms = self._sms(combine=True)
+        args = (x.data_ptr(), idx, topk_weights.data_ptr(), send_pos.data_ptr(),
+                shared.data_ptr() if shared is not None else 0, residual.data_ptr(), residual_out.data_ptr(),
+                weight.data_ptr(), out.data_ptr(), scales.data_ptr() if scales is not None else 0, T, H, K, E, M,
+                float(eps), sms)
+        hook = None
+        if return_recv_hook:
+            # SEND half: (pack the expert outputs into the symmetric buffer and) announce that they are in place
+            self.rt.ll_combine_rmsnorm(*args, st.cuda_stream, phase=C.EP_LL_SEND, layout_range=layout_range.data_ptr(),
+                                       wait_stats=stats_ptr, use_logfmt=bool(use_logfmt))
+
+            sent = torch.cuda.Event()
+            sent.record(st)
+
+            def hook():
+                if self._pending is hook:
+                    self._pending = None
+                    with torch.cuda.device(dev):
+                        cur = torch.cuda.current_stream(dev)
+                        cur.wait_event(sent)  # see dispatch: epoch hand-over between the two halves
+                        self.rt.ll_combine_rmsnorm(*args, cur.cuda_stream, phase=C.EP_LL_RECV,
+                                                   layout_range=layout_range.data_ptr(), wait_stats=stats_ptr)
+
+            # alive until the receive half has run
+            hook._keep = (x, topk_weights, send_pos, shared, residual, residual_out, weight, out, scales, layout_range,
+                          combine_wait_recv_cost_stats)
+            self._pending = hook
+        else:
+            self.rt.ll_combine_rmsnorm(*args, st.cuda_stream, phase=C.EP_LL_FULL, layout_range=layout_range.data_ptr(),
+                                       wait_stats=stats_ptr, use_logfmt=bool(use_logfmt))
+        ev = EventOverlap(EventHandle(st)) if async_finish else EventOverlap()
+        return ((out, scales) if scales is not None else out), ev, hook
