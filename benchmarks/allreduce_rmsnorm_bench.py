@@ -102,28 +102,6 @@ def run_ep(a, rank, n, dev, dist, info):
     w = (torch.rand(H, generator=g) + 0.5).to(torch.bfloat16).to(dev)
     rows = []
 
-    def graph_of(fn):
-        for _ in range(a.warmup):
-            fn()
-        torch.cuda.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            for _ in range(a.iters):
-                fn()
-        graph.replay()
-        torch.cuda.synchronize()
-        return graph
-
-    def replay_us(graph):
-        if dist is not None:
-            dist.barrier()
-        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        s.record()
-        graph.replay()
-        e.record()
-        torch.cuda.synchronize()
-        return mx(s.elapsed_time(e) / a.iters * 1e3, dist, dev)
-
     for T in tokens:
         x = torch.randn(T, H, generator=g).to(torch.bfloat16).to(dev)
         idx = torch.rand(T, E, generator=g).topk(K, dim=1).indices.to(torch.int64).to(dev)
@@ -160,11 +138,11 @@ def run_ep(a, rank, n, dev, dist, info):
                     for p, q in zip(yf if fp8 else (yf,), yu if fp8 else (yu,)))
                 if not same:
                     raise SystemExit(f"--mode ep: fused and unfused outputs differ (T={T}, num_sms={sms}, fp8={fp8})")
-                graphs = {"fused": graph_of(fused), "unfused": graph_of(unfused), "torch": graph_of(torch_tail)}
+                graphs = {k: graph_of(fn, a) for k, fn in (("fused", fused), ("unfused", unfused), ("torch", torch_tail))}
                 times = {k: [] for k in graphs}
                 for _ in range(a.rounds):  # alternate the arms so drift and neighbours hit them alike
                     for k, gr in graphs.items():
-                        times[k].append(replay_us(gr))
+                        times[k].append(replay_us(gr, a, dist, dev))
                 del graphs
                 row = {"mode": "ep", "T": T, "num_recv": num_recv, "H": H, "topk": K, "experts": E, "fp8": fp8,
                        "num_sms": sms, "n_gpus": n, "bitwise_fused_eq_unfused": same}
@@ -215,28 +193,6 @@ def run_ll(a, rank, n, dev, dist, info):
     w = (torch.rand(H, generator=g) + 0.5).to(torch.bfloat16).to(dev)
     rows = []
 
-    def graph_of(fn):
-        for _ in range(a.warmup):
-            fn()
-        torch.cuda.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            for _ in range(a.iters):
-                fn()
-        graph.replay()
-        torch.cuda.synchronize()
-        return graph
-
-    def replay_us(graph):
-        if dist is not None:
-            dist.barrier()
-        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        s.record()
-        graph.replay()
-        e.record()
-        torch.cuda.synchronize()
-        return mx(s.elapsed_time(e) / a.iters * 1e3, dist, dev)
-
     for T in tokens:
         x = torch.randn(T, H, generator=g).to(torch.bfloat16).to(dev)
         idx = torch.rand(T, E, generator=g).topk(K, dim=1).indices.to(torch.int64).to(dev)
@@ -272,11 +228,11 @@ def run_ll(a, rank, n, dev, dist, info):
                 for p, q in zip(yf if fp8 else (yf,), yu if fp8 else (yu,)))
             if not same:
                 raise SystemExit(f"--mode ll: fused and unfused outputs differ (T={T}, fp8={fp8})")
-            graphs = {"fused": graph_of(fused), "unfused": graph_of(unfused), "torch": graph_of(torch_tail)}
+            graphs = {k: graph_of(fn, a) for k, fn in (("fused", fused), ("unfused", unfused), ("torch", torch_tail))}
             times = {k: [] for k in graphs}
             for _ in range(a.rounds):  # alternate the arms so drift and neighbours hit them alike
                 for k, gr in graphs.items():
-                    times[k].append(replay_us(gr))
+                    times[k].append(replay_us(gr, a, dist, dev))
             del graphs
             row = {"mode": "ll", "T": T, "routed_rows": routed_rows, "H": H, "topk": K, "experts": E, "M": M,
                    "fp8": fp8, "n_gpus": n, "bitwise_fused_eq_unfused": same, **info}
@@ -300,6 +256,33 @@ def mx(v, dist, dev):
     t = torch.tensor([v], dtype=torch.float64, device=dev)
     dist.all_reduce(t, op=dist.ReduceOp.MAX)
     return float(t.item())
+
+
+def graph_of(fn, a):
+    """--iters calls of fn captured in one CUDA graph, after --warmup eager calls and one replay: at these sizes
+    enqueuing a call from Python takes longer than the GPU takes to run it, and eager timing would measure the host."""
+    for _ in range(a.warmup):
+        fn()
+    torch.cuda.synchronize()
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        for _ in range(a.iters):
+            fn()
+    graph.replay()
+    torch.cuda.synchronize()
+    return graph
+
+
+def replay_us(graph, a, dist, dev):
+    """Microseconds per call of one replay of graph_of's graph, the slowest rank's."""
+    if dist is not None:
+        dist.barrier()
+    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    s.record()
+    graph.replay()
+    e.record()
+    torch.cuda.synchronize()
+    return mx(s.elapsed_time(e) / a.iters * 1e3, dist, dev)
 
 
 def main():
@@ -355,33 +338,8 @@ def main():
     else:
         comm = Communicator.local_world(1, devices=[0], heap_bytes=512 << 20, stage_bytes=64 << 20)[0]
 
-    def mx(v):
-        if dist is None:
-            return v
-        t = torch.tensor([v], dtype=torch.float64, device=dev)
-        dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        return float(t.item())
-
     def timed(fn):
-        # --iters calls captured in one CUDA graph: at these sizes enqueuing a call from Python takes longer than
-        # the GPU takes to run it, and eager timing would measure the host
-        for _ in range(a.warmup):
-            fn()
-        torch.cuda.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            for _ in range(a.iters):
-                fn()
-        graph.replay()
-        torch.cuda.synchronize()
-        if dist is not None:
-            dist.barrier()
-        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        s.record()
-        graph.replay()
-        e.record()
-        torch.cuda.synchronize()
-        return mx(s.elapsed_time(e) / a.iters) * 1e3
+        return replay_us(graph_of(fn, a), a, dist, dev)
 
     rows = []
     g = torch.Generator(device="cpu").manual_seed(rank)

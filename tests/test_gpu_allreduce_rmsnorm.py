@@ -6,7 +6,7 @@ import pytest
 import torch
 
 from helpers import get_world, run_ranks
-from uccl_b200.ep.utils import per_token_cast_to_fp8
+from rmsnorm_ref import assert_fp8_cast_of, rmsnorm_ref
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(600)]
 
@@ -76,9 +76,7 @@ def test_allreduce_rmsnorm(n, dtype, T, H, sym, separate):
         assert torch.equal(x, ref_x[r])
         # 2. residual_out and out against fp64
         assert torch.allclose(ro.double(), x.double() + residual.double(), **_tol(dtype))
-        rr = ro.double()
-        ref_y = rr * torch.rsqrt(rr.pow(2).mean(1, keepdim=True) + EPS) * weight.double()
-        assert torch.allclose(y.double(), ref_y, **_tol(dtype))
+        assert torch.allclose(y.double(), rmsnorm_ref(ro, weight, EPS), **_tol(dtype))
         # 3. bitwise identical on every rank
         assert torch.equal(x, res[0][0]) and torch.equal(ro, res[0][1]) and torch.equal(y, res[0][2])
 
@@ -95,9 +93,7 @@ def test_allreduce_rmsnorm(n, dtype, T, H, sym, separate):
     q8 = _run(comms, xs, residual, weight, sym, separate, quant="fp8")
     for (x, ro, y), (x8, ro8, (q, sc)) in zip(res, q8):
         assert torch.equal(x, x8) and torch.equal(ro, ro8)
-        q_ref, sc_ref = per_token_cast_to_fp8(y)
-        assert torch.equal(q.view(torch.uint8), q_ref.view(torch.uint8))
-        assert torch.equal(sc, sc_ref)
+        assert_fp8_cast_of(q, sc, y)
         assert q.dtype == torch.float8_e4m3fn and sc.dtype == torch.float32
         assert sc.is_contiguous() and sc.shape == (q.size(0), q.size(1) // 128)
 
@@ -127,9 +123,7 @@ def test_allreduce_rmsnorm_interleaved_with_oneshot_allreduce(n):
             assert torch.allclose(s["p"].cpu().double(), exp_p, rtol=1e-5, atol=1e-5), rnd
             assert torch.equal(s["p"].cpu(), s["p2"].cpu()), rnd
             assert torch.allclose(s["x"].cpu().double(), exp_x.double(), **_tol(dtype)), rnd
-            rr = s["res"].cpu().double()
-            ref_y = rr * torch.rsqrt(rr.pow(2).mean(1, keepdim=True) + EPS) * weight.double()
-            assert torch.allclose(s["y"].cpu().double(), ref_y, **_tol(dtype)), rnd
+            assert torch.allclose(s["y"].cpu().double(), rmsnorm_ref(s["res"].cpu(), weight, EPS), **_tol(dtype)), rnd
 
 
 def test_allreduce_rmsnorm_cuda_graph_replay():
@@ -168,6 +162,4 @@ def test_allreduce_rmsnorm_cuda_graph_replay():
         for x, r, y in zip(xs, rs, ys):
             assert torch.equal(x.cpu(), exp_x), rep
             assert torch.equal(r.cpu(), (exp_x.float() + residual.float()).to(dtype)), rep
-            rr = r.cpu().double()
-            ref_y = rr * torch.rsqrt(rr.pow(2).mean(1, keepdim=True) + EPS) * weight.double()
-            assert torch.allclose(y.cpu().double(), ref_y, **_tol(dtype)), rep
+            assert torch.allclose(y.cpu().double(), rmsnorm_ref(r.cpu(), weight, EPS), **_tol(dtype)), rep

@@ -5,9 +5,9 @@ tokens routed to no rank, the launch count, interleaving with dispatch / combine
 import pytest
 import torch
 
-from helpers import get_world
+from rmsnorm_ref import assert_fp8_cast_of, one_rank_epilogue
 from test_gpu_ep import get_buffers, make_inputs, run_threads
-from uccl_b200.ep.utils import EpHandle, per_token_cast_to_fp8
+from uccl_b200.ep.utils import EpHandle
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
@@ -55,31 +55,18 @@ def _dispatch(b, x, idx, E):
     return recv_x, handle
 
 
-def _expected(combined, residual, weight, quant):
-    """combine() followed by the epilogue kernel of a one-rank all_reduce_rmsnorm (add_rmsnorm_kernel)."""
-    c1 = get_world(1)[0]
-    dev = c1.device
-    x, ro = combined.to(dev), residual.to(dev)
-    y = c1.all_reduce_rmsnorm(x, ro, weight.to(dev), EPS)
-    y = y.cpu()
-    # on the host, like the other fp8 tests: torch's CUDA division by a scalar multiplies by its reciprocal instead
-    q = per_token_cast_to_fp8(y) if quant == "fp8" else None
-    return ro.cpu(), y, q
-
-
 def _check(got_ro, got_y, combined, residual, weight, quant, what):
     if combined.size(0) == 0:  # a rank without tokens: nothing to compare, but it joined every call
         assert got_ro.shape == combined.shape, what
         assert (got_y[0] if quant == "fp8" else got_y).shape == combined.shape, what
         return
-    ro, y, q = _expected(combined, residual, weight, quant)
+    ro, y, q = one_rank_epilogue(combined, residual, weight, EPS, quant)  # combine(), then the unfused epilogue
     assert torch.equal(got_ro, ro), what
     if quant == "fp8":
         gq, gs = got_y
         assert gq.dtype == torch.float8_e4m3fn and gs.dtype == torch.float32, what
         assert gs.shape == (y.size(0), y.size(1) // 128), what
-        assert torch.equal(gq.view(torch.uint8), q[0].view(torch.uint8)), what
-        assert torch.equal(gs, q[1]), what
+        assert_fp8_cast_of(gq, gs, y, what)
     else:
         assert torch.equal(got_y, y), what
 

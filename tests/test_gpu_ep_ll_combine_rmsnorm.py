@@ -7,9 +7,9 @@ import pytest
 import torch
 
 from helpers import get_world
+from rmsnorm_ref import assert_fp8_cast_of, one_rank_epilogue
 from test_gpu_ep import run_threads
 from uccl_b200.ep import Buffer
-from uccl_b200.ep.utils import per_token_cast_to_fp8
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
@@ -62,31 +62,20 @@ def _experts(rx, r):
     return (rx.float() * f).to(torch.bfloat16)
 
 
-def _expected(routed, shared, residual, weight, quant):
-    """torch's bf16 routed + shared, then the epilogue kernel of a one-rank all_reduce_rmsnorm (add_rmsnorm_kernel)."""
-    c1 = get_world(1)[0]
-    dev = c1.device
-    x = routed.to(dev) if shared is None else routed.to(dev) + shared.to(dev)
-    ro = residual.to(dev).clone()
-    y = c1.all_reduce_rmsnorm(x, ro, weight.to(dev), EPS).cpu()
-    # on the host, like the other fp8 tests: torch's CUDA division by a scalar multiplies by its reciprocal instead
-    q = per_token_cast_to_fp8(y) if quant == "fp8" else None
-    return ro.cpu(), y, q
-
-
 def _check(got_ro, got_y, routed, shared, residual, weight, quant, what):
     T = got_ro.size(0)
     if T == 0:  # a rank without tokens: nothing to compare, but it joined every call
         assert (got_y[0] if quant == "fp8" else got_y).size(0) == 0, what
         return
-    ro, y, q = _expected(routed[:T], shared, residual[:T], weight, quant)
+    # torch's bf16 routed + shared, then the unfused epilogue
+    x = routed[:T].cuda() if shared is None else routed[:T].cuda() + shared.cuda()
+    ro, y, q = one_rank_epilogue(x, residual[:T], weight, EPS, quant)
     assert torch.equal(got_ro, ro), what
     if quant == "fp8":
         gq, gs = got_y
         assert gq.dtype == torch.float8_e4m3fn and gs.dtype == torch.float32, what
         assert gs.shape == (T, y.size(1) // 128), what
-        assert torch.equal(gq.view(torch.uint8), q[0].view(torch.uint8)), what
-        assert torch.equal(gs, q[1]), what
+        assert_fp8_cast_of(gq, gs, y, what)
     else:
         assert torch.equal(got_y, y), what
 

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from helpers import get_world, run_ranks
-from uccl_b200.ep.utils import per_token_cast_to_fp8
+from rmsnorm_ref import assert_fp8_cast_of, rmsnorm_ref
 from uccl_b200.parallel.comm import launch_count
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
@@ -33,11 +33,6 @@ def _rank_order_sum(xs):
     for x in xs[1:]:
         acc = acc + x.float()
     return acc.to(xs[0].dtype)
-
-
-def _rmsnorm_ref(ro, weight):
-    rr = ro.double()
-    return rr * torch.rsqrt(rr.pow(2).mean(1, keepdim=True) + EPS) * weight.double()
 
 
 def _place(c, t, sym):
@@ -127,7 +122,7 @@ def test_reduce_scatter_rmsnorm(n, dtype, Tl, H, sym):
         # 2. residual_out and out against fp64
         assert ro.shape == (Tl, H) and y.shape == (Tl, H)
         assert torch.allclose(ro.double(), x[lo:hi].double() + residual[lo:hi].double(), **_tol(dtype))
-        assert torch.allclose(y.double(), _rmsnorm_ref(ro, weight), **_tol(dtype))
+        assert torch.allclose(y.double(), rmsnorm_ref(ro, weight, EPS), **_tol(dtype))
 
     # 3. SP == TP: the shards in rank order are what all_reduce_rmsnorm gives on the same x with the full residual
     ro_tp, y_tp = _tp(comms, xs, residual, weight, sym)
@@ -138,9 +133,7 @@ def test_reduce_scatter_rmsnorm(n, dtype, Tl, H, sym):
     q8 = _sp(comms, xs, residual, weight, sym, separate, quant="fp8")
     for (x, ro, y), (x8, ro8, (q, sc)) in zip(res, q8):
         assert torch.equal(x, x8) and torch.equal(ro, ro8)
-        q_ref, sc_ref = per_token_cast_to_fp8(y)
-        assert torch.equal(q.view(torch.uint8), q_ref.view(torch.uint8))
-        assert torch.equal(sc, sc_ref)
+        assert_fp8_cast_of(q, sc, y)
         assert q.dtype == torch.float8_e4m3fn and sc.dtype == torch.float32
         assert sc.is_contiguous() and sc.shape == (Tl, H // 128)
     _, (q_tp, sc_tp) = _tp(comms, xs, residual, weight, sym, quant="fp8")
@@ -207,7 +200,7 @@ def test_reduce_scatter_rmsnorm_interleaved_with_ll_collectives(n):
                 xr = _rank_order_sum(x_in)[sl]
                 assert torch.equal(s[xk].cpu()[sl], xr), (rnd, xk)
                 assert torch.equal(s[rk].cpu(), (xr.float() + res_in[sl].float()).to(dtype)), (rnd, xk)
-                assert torch.allclose(s[yk].cpu().double(), _rmsnorm_ref(s[rk].cpu(), weight), **_tol(dtype)), rnd
+                assert torch.allclose(s[yk].cpu().double(), rmsnorm_ref(s[rk].cpu(), weight, EPS), **_tol(dtype)), rnd
         # the interleaved TP call agrees with the SP calls around it
         assert torch.equal(torch.cat([s["y"].cpu() for s in states]), states[0]["ty"].cpu()), rnd
 
@@ -254,4 +247,4 @@ def test_reduce_scatter_rmsnorm_cuda_graph_replay():
             assert torch.equal(xc[sl], exp_x[sl]), rep
             assert torch.equal(xc[:lo], ins[k][:lo]) and torch.equal(xc[hi:], ins[k][hi:]), rep
             assert torch.equal(r.cpu(), (exp_x[sl].float() + residual[sl].float()).to(dtype)), rep
-            assert torch.allclose(y.cpu().double(), _rmsnorm_ref(r.cpu(), weight), **_tol(dtype)), rep
+            assert torch.allclose(y.cpu().double(), rmsnorm_ref(r.cpu(), weight, EPS), **_tol(dtype)), rep

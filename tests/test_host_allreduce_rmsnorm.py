@@ -4,8 +4,8 @@ import pytest
 import torch
 
 from helpers import run_host_ranks
+from rmsnorm_ref import assert_fp8_cast_of, rmsnorm_ref
 from uccl_b200 import Communicator
-from uccl_b200.ep.utils import per_token_cast_to_fp8
 
 N = 4
 EPS = 1e-6
@@ -51,9 +51,7 @@ def test_host_allreduce_rmsnorm_matches_fp64_reference(world4, dtype, separate, 
         assert torch.allclose(ro.double(), ref_ro, **_tol(dtype))
         if separate:
             assert torch.equal(res, residual)  # residual itself untouched
-        r = ro.double()
-        ref_y = r * torch.rsqrt(r.pow(2).mean(1, keepdim=True) + EPS) * weight.double()
-        assert torch.allclose(y.double(), ref_y, **_tol(dtype))
+        assert torch.allclose(y.double(), rmsnorm_ref(ro, weight, EPS), **_tol(dtype))
     for x, _, ro, y in outs[1:]:  # every rank holds the same bits
         assert torch.equal(x, outs[0][0]) and torch.equal(ro, outs[0][2]) and torch.equal(y, outs[0][3])
 
@@ -69,9 +67,7 @@ def test_host_allreduce_rmsnorm_fp8_is_per_token_cast_of_out(world4, dtype, sepa
         assert torch.equal(x0, x1) and torch.equal(ro0, ro1)
         assert q.dtype == torch.float8_e4m3fn and q.shape == (T, H)
         assert sc.dtype == torch.float32 and sc.shape == (T, H // 128)
-        q_ref, sc_ref = per_token_cast_to_fp8(y0)
-        assert torch.equal(q.view(torch.uint8), q_ref.view(torch.uint8))
-        assert torch.equal(sc, sc_ref)
+        assert_fp8_cast_of(q, sc, y0)
 
 
 def test_host_allreduce_rmsnorm_argument_checks(world4):

@@ -5,9 +5,9 @@ import pytest
 import torch
 
 from helpers import run_host_ranks
+from rmsnorm_ref import assert_fp8_cast_of, rmsnorm_ref
 from uccl_b200 import Communicator
 from uccl_b200.ep import Buffer
-from uccl_b200.ep.utils import per_token_cast_to_fp8
 
 N = 4
 EPS = 1e-6
@@ -77,7 +77,7 @@ def test_host_combine_rmsnorm_matches_fp64_reference(world4, bias_mode, separate
             if bb is not None:
                 ref_c = ref_c + bb.double()
         ref_ro = ref_c + residuals[r].double()
-        ref_y = ref_ro * torch.rsqrt(ref_ro.pow(2).mean(1, keepdim=True) + EPS) * weight.double()
+        ref_y = rmsnorm_ref(ref_ro, weight, EPS)
         assert torch.allclose(ro.double(), ref_ro, **tol)
         assert torch.allclose(y.double(), ref_y, **tol)
         # residual_out is bf16(combine() + residual) exactly
@@ -98,9 +98,7 @@ def test_host_combine_rmsnorm_fp8_is_per_token_cast_of_out(world4, separate):
         assert q.dtype == torch.float8_e4m3fn and q.shape == (Ts[r], H)
         assert sc.dtype == torch.float32 and sc.shape == (Ts[r], H // 128) and sc.is_contiguous()
         if Ts[r]:
-            q_ref, sc_ref = per_token_cast_to_fp8(y0)
-            assert torch.equal(q.view(torch.uint8), q_ref.view(torch.uint8))
-            assert torch.equal(sc, sc_ref)
+            assert_fp8_cast_of(q, sc, y0)
 
 
 def test_host_combine_rmsnorm_rank_without_tokens(world4):

@@ -6,9 +6,9 @@ import pytest
 import torch
 
 from helpers import run_host_ranks
+from rmsnorm_ref import assert_fp8_cast_of, rmsnorm_ref
 from uccl_b200 import Communicator, _native
 from uccl_b200.ep import Buffer
-from uccl_b200.ep.utils import per_token_cast_to_fp8
 from uccl_b200.parallel.comm import dtype_code
 
 N = 4
@@ -108,7 +108,7 @@ def test_host_ll_combine_rmsnorm_matches_unfused_and_fp64(world4, with_shared, s
         if with_shared:
             ref = ref + shared.double()
         ref_ro = ref + residuals[r].double()
-        ref_y = ref_ro * torch.rsqrt(ref_ro.pow(2).mean(1, keepdim=True) + EPS) * weight.double()
+        ref_y = rmsnorm_ref(ref_ro, weight, EPS)
         assert torch.allclose(ro.double(), ref_ro, rtol=2e-2, atol=5e-2)
         assert torch.allclose(y.double(), ref_y, rtol=2e-2, atol=5e-2)
 
@@ -123,9 +123,7 @@ def test_host_ll_combine_rmsnorm_fp8_is_per_token_cast_of_out(world4, with_share
         assert torch.equal(ro0, ro1)
         assert q.dtype == torch.float8_e4m3fn and q.shape == (Ts[r], H)
         assert sc.dtype == torch.float32 and sc.shape == (Ts[r], H // 128) and sc.is_contiguous()
-        q_ref, sc_ref = per_token_cast_to_fp8(y0)
-        assert torch.equal(q.view(torch.uint8), q_ref.view(torch.uint8))
-        assert torch.equal(sc, sc_ref)
+        assert_fp8_cast_of(q, sc, y0)
         _, (q_u, sc_u) = _unfused(routed, shareds[r] if with_shared else None, residuals[r], weight, True)
         assert torch.equal(q.view(torch.uint8), q_u.view(torch.uint8)) and torch.equal(sc, sc_u)
 

@@ -5,8 +5,8 @@ import pytest
 import torch
 
 from helpers import run_host_ranks
+from rmsnorm_ref import assert_fp8_cast_of, rmsnorm_ref
 from uccl_b200 import Communicator
-from uccl_b200.ep.utils import per_token_cast_to_fp8
 
 N = 4
 EPS = 1e-6
@@ -61,9 +61,7 @@ def test_host_reduce_scatter_rmsnorm_matches_fp64_reference(world4, dtype, separ
         assert torch.allclose(ro.double(), xr.double() + residual[lo:hi].double(), **_tol(dtype))
         if separate:
             assert torch.equal(res, residual[lo:hi])  # the residual shard itself is untouched
-        rr = ro.double()
-        ref_y = rr * torch.rsqrt(rr.pow(2).mean(1, keepdim=True) + EPS) * weight.double()
-        assert torch.allclose(y.double(), ref_y, **_tol(dtype))
+        assert torch.allclose(y.double(), rmsnorm_ref(ro, weight, EPS), **_tol(dtype))
         assert y.shape == (Tl, H)
 
 
@@ -94,9 +92,7 @@ def test_host_reduce_scatter_rmsnorm_fp8_is_per_token_cast_of_out(world4, dtype,
         assert torch.equal(x0, x1) and torch.equal(ro0, ro1)
         assert q.dtype == torch.float8_e4m3fn and q.shape == (T // N, H)
         assert sc.dtype == torch.float32 and sc.shape == (T // N, H // 128) and sc.is_contiguous()
-        q_ref, sc_ref = per_token_cast_to_fp8(y0)
-        assert torch.equal(q.view(torch.uint8), q_ref.view(torch.uint8))
-        assert torch.equal(sc, sc_ref)
+        assert_fp8_cast_of(q, sc, y0)
 
 
 def test_host_reduce_scatter_rmsnorm_argument_checks(world4):

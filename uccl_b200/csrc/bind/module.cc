@@ -46,8 +46,9 @@ PYBIND11_MODULE(_C, m) {
       "host_add_rmsnorm",
       [](uintptr_t x, uintptr_t residual, uintptr_t residual_out, uintptr_t weight, uintptr_t out, uintptr_t out_scales,
          size_t T, size_t H, int dtype, float eps) {
-        UB_CHECK(dtype == kBF16 || dtype == kF16, "host_add_rmsnorm: dtype must be bf16 or fp16 (got %d)", dtype);
-        UB_CHECK(!out_scales || H % 128 == 0, "host_add_rmsnorm: fp8 output needs hidden size %% 128 == 0");
+        rmsnorm_tail_args("host_add_rmsnorm", P(x), P(residual), P(residual_out), P(weight), P(out),
+                          reinterpret_cast<float*>(out_scales), (int64_t)T, (int64_t)H, dtype, eps, out_scales != 0,
+                          kRmsMaxH, 8, false);
         py::gil_scoped_release rel;
         host_add_rmsnorm(P(x), P(residual), P(residual_out), P(weight), P(out), reinterpret_cast<float*>(out_scales), T,
                          H, dtype, eps);

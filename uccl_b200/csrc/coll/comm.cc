@@ -469,43 +469,61 @@ void Comm::allreduce(const void* in, void* out, size_t count, int dtype, int op,
 }
 
 // ---------------------------------------------------------- allreduce + rmsnorm
-void Comm::allreduce_rmsnorm(void* x, const void* residual, void* residual_out, const void* weight, void* out,
-                             float* out_scales, size_t T, size_t H, int dtype, float eps, int quant,
-                             cudaStream_t stream, const ArOpts& opts) {
-  UB_CHECK(dtype == kBF16 || dtype == kF16, "allreduce_rmsnorm: dtype must be bf16 or fp16 (got %d)", dtype);
-  UB_CHECK(H >= 8 && H <= kRmsMaxH && H % 8 == 0, "allreduce_rmsnorm: hidden size %zu must be a multiple of 8 in [8, %u]",
-           H, kRmsMaxH);
-  UB_CHECK(quant == 0 || quant == 1, "allreduce_rmsnorm: bad quant %d", quant);
-  UB_CHECK(!quant || H % 128 == 0, "allreduce_rmsnorm: fp8 output needs hidden size %% 128 == 0 (got %zu)", H);
-  UB_CHECK(T <= UINT32_MAX, "allreduce_rmsnorm: too many rows (%zu)", T);
-  if (T == 0) return;
-  check_buf(x, "x");
-  check_buf(residual, "residual");
-  check_buf(residual_out, "residual_out");
-  check_buf(weight, "weight");
-  check_buf(out, "out");
-  if (quant) check_buf(out_scales, "out_scales");
-  float* scales = quant ? out_scales : nullptr;
-  const int n = nranks();
-  const size_t count = T * H, bytes = count * dtype_size(dtype);
-  if (is_host()) {
-    host_allreduce(x, x, count, dtype, kSum, 1.0f, dtype);
-    host_add_rmsnorm(x, residual, residual_out, weight, out, scales, T, H, dtype, eps);
-    return;
+RmsNormArgs rmsnorm_tail_args(const char* op, void* x, const void* residual, void* residual_out, const void* weight,
+                              void* out, float* out_scales, int64_t T, int64_t H, int dtype, float eps, bool fp8,
+                              uint32_t max_h, uint32_t mult, bool aligned, std::initializer_list<const void*> extra) {
+  UB_CHECK(dtype == kBF16 || dtype == kF16, "%s: dtype must be bf16 or fp16 (got %d)", op, dtype);
+  UB_CHECK(H >= mult && H <= max_h && H % mult == 0, "%s: hidden size %lld must be a multiple of %u in [%u, %u]", op,
+           (long long)H, mult, mult, max_h);
+  UB_CHECK(!fp8 || H % 128 == 0, "%s: fp8 output needs hidden size %% 128 == 0 (got %lld)", op, (long long)H);
+  UB_CHECK(T >= 0 && T <= UINT32_MAX, "%s: bad row count %lld", op, (long long)T);
+  if (!fp8) out_scales = nullptr;
+  UB_CHECK(T == 0 || (residual && residual_out && weight && out && (!fp8 || out_scales)),
+           "%s: residual, residual_out, weight, out or out_scales is null", op);
+  if (aligned) {
+    uintptr_t bits = (uintptr_t)x | (uintptr_t)residual | (uintptr_t)residual_out | (uintptr_t)weight |
+                     (uintptr_t)out | (uintptr_t)out_scales;
+    for (const void* p : extra) bits |= (uintptr_t)p;
+    UB_CHECK((bits & 15) == 0, "%s: every tensor must be 16-byte aligned", op);
   }
-  DeviceGuard g(device());
-  UB_CHECK(aligned16(x) && aligned16(residual) && aligned16(residual_out) && aligned16(weight) && aligned16(out),
-           "allreduce_rmsnorm: x, residual, residual_out, weight and out must be 16-byte aligned");
   RmsNormArgs r;
   r.x = x;
   r.residual = residual;
   r.residual_out = residual_out;
   r.weight = weight;
   r.out = out;
-  r.out_scales = scales;
+  r.out_scales = out_scales;
   r.T = (uint32_t)T;
   r.H = (uint32_t)H;
   r.eps = eps;
+  return r;
+}
+
+void Comm::launch_add_rmsnorm(const RmsNormArgs& r, int dtype, bool fp8, cudaStream_t stream) {
+  const int grid = (int)std::min<uint32_t>(r.T, 1024);
+  cudaError_t e = launch_allreduce_rmsnorm(0, dtype, fp8, dev_, base_args(), r, grid, stream);
+  UB_CHECK(e == cudaSuccess, "add_rmsnorm launch failed (rank %d): %s", rank(), cudaGetErrorString(e));
+  ++launches_;
+}
+
+void Comm::allreduce_rmsnorm(void* x, const void* residual, void* residual_out, const void* weight, void* out,
+                             float* out_scales, size_t T, size_t H, int dtype, float eps, int quant,
+                             cudaStream_t stream, const ArOpts& opts) {
+  UB_CHECK(quant == 0 || quant == 1, "allreduce_rmsnorm: bad quant %d", quant);
+  UB_CHECK(T == 0 || x, "allreduce_rmsnorm: x is null");
+  // the host epilogue has never needed aligned rows
+  const RmsNormArgs r = rmsnorm_tail_args("allreduce_rmsnorm", x, residual, residual_out, weight, out, out_scales,
+                                          (int64_t)T, (int64_t)H, dtype, eps, quant != 0, kRmsMaxH, 8,
+                                          T > 0 && !is_host());
+  if (T == 0) return;
+  const int n = nranks();
+  const size_t count = T * H, bytes = count * dtype_size(dtype);
+  if (is_host()) {
+    host_allreduce(x, x, count, dtype, kSum, 1.0f, dtype);
+    host_add_rmsnorm(x, residual, residual_out, weight, out, r.out_scales, T, H, dtype, eps);
+    return;
+  }
+  DeviceGuard g(device());
 
   // the fused kernel takes exactly the sizes for which the plain all-reduce would run one-shot
   int algo = opts.algo, ctas = 0;
@@ -535,10 +553,7 @@ void Comm::allreduce_rmsnorm(void* x, const void* residual, void* residual_out, 
     o.max_ctas = opts.max_ctas;
     allreduce(x, x, count, dtype, kSum, stream, o);
   }
-  const int grid = (int)std::min<size_t>(T, 1024);
-  cudaError_t e = launch_allreduce_rmsnorm(0, dtype, quant != 0, dev_, base_args(), r, grid, stream);
-  UB_CHECK(e == cudaSuccess, "add_rmsnorm launch failed (rank %d): %s", rank(), cudaGetErrorString(e));
-  ++launches_;
+  launch_add_rmsnorm(r, dtype, quant != 0, stream);
   UB_TRACE(SUB_COLL, "allreduce_rmsnorm unfused T=%zu H=%zu algo=%s", T, H, algo_name(algo));
 }
 
@@ -546,42 +561,23 @@ void Comm::allreduce_rmsnorm(void* x, const void* residual, void* residual_out, 
 void Comm::reduce_scatter_rmsnorm(void* x, const void* residual, void* residual_out, const void* weight, void* out,
                                   float* out_scales, size_t T, size_t H, int dtype, float eps, int quant,
                                   cudaStream_t stream) {
-  UB_CHECK(dtype == kBF16 || dtype == kF16, "reduce_scatter_rmsnorm: dtype must be bf16 or fp16 (got %d)", dtype);
-  UB_CHECK(H >= 8 && H <= kRmsMaxH && H % 8 == 0,
-           "reduce_scatter_rmsnorm: hidden size %zu must be a multiple of 8 in [8, %u]", H, kRmsMaxH);
   UB_CHECK(quant == 0 || quant == 1, "reduce_scatter_rmsnorm: bad quant %d", quant);
-  UB_CHECK(!quant || H % 128 == 0, "reduce_scatter_rmsnorm: fp8 output needs hidden size %% 128 == 0 (got %zu)", H);
-  UB_CHECK(T <= UINT32_MAX, "reduce_scatter_rmsnorm: too many rows (%zu)", T);
   const int n = nranks();
   UB_CHECK(T % n == 0, "reduce_scatter_rmsnorm: %zu tokens do not split evenly over %d ranks", T, n);
-  if (T == 0) return;
-  check_buf(x, "x");
-  check_buf(residual, "residual");
-  check_buf(residual_out, "residual_out");
-  check_buf(weight, "weight");
-  check_buf(out, "out");
-  if (quant) check_buf(out_scales, "out_scales");
-  float* scales = quant ? out_scales : nullptr;
+  UB_CHECK(T == 0 || x, "reduce_scatter_rmsnorm: x is null");
   const size_t Tl = T / n, count = Tl * H, bytes = count * dtype_size(dtype);  // one rank's piece
   char* own = static_cast<char*>(x) + (size_t)rank() * bytes;
+  // the host epilogue has never needed aligned rows
+  const RmsNormArgs r = rmsnorm_tail_args("reduce_scatter_rmsnorm", own, residual, residual_out, weight, out,
+                                          out_scales, (int64_t)Tl, (int64_t)H, dtype, eps, quant != 0, kRmsMaxH, 8,
+                                          T > 0 && !is_host());
+  if (T == 0) return;
   if (is_host()) {
     host_reduce_scatter(x, own, count, dtype, kSum);  // stages every piece before it reduces: in place is safe
-    host_add_rmsnorm(own, residual, residual_out, weight, out, scales, Tl, H, dtype, eps);
+    host_add_rmsnorm(own, residual, residual_out, weight, out, r.out_scales, Tl, H, dtype, eps);
     return;
   }
   DeviceGuard g(device());
-  UB_CHECK(aligned16(x) && aligned16(residual) && aligned16(residual_out) && aligned16(weight) && aligned16(out),
-           "reduce_scatter_rmsnorm: x, residual, residual_out, weight and out must be 16-byte aligned");
-  RmsNormArgs r;
-  r.x = own;
-  r.residual = residual;
-  r.residual_out = residual_out;
-  r.weight = weight;
-  r.out = out;
-  r.out_scales = scales;
-  r.T = (uint32_t)Tl;
-  r.H = (uint32_t)H;
-  r.eps = eps;
 
   // the fused kernel takes exactly the sizes for which the plain reduce_scatter would run the LL kernel
   // (bytes % 16 == 0 because H % 8 == 0), with that kernel's grid
@@ -602,10 +598,7 @@ void Comm::reduce_scatter_rmsnorm(void* x, const void* residual, void* residual_
   // in place: every reduce_scatter kernel reads the own piece of its input before (or, per unit, as) it writes the
   // result over it, and peers only read their own pieces (see rs_kernel)
   if (n > 1) reduce_scatter(x, own, count, dtype, kSum, stream);
-  const int grid = (int)std::min<size_t>(Tl, 1024);
-  cudaError_t e = launch_allreduce_rmsnorm(0, dtype, quant != 0, dev_, base_args(), r, grid, stream);
-  UB_CHECK(e == cudaSuccess, "add_rmsnorm launch failed (rank %d): %s", rank(), cudaGetErrorString(e));
-  ++launches_;
+  launch_add_rmsnorm(r, dtype, quant != 0, stream);
   UB_TRACE(SUB_COLL, "reduce_scatter_rmsnorm unfused T=%zu H=%zu", T, H);
 }
 

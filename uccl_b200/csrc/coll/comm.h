@@ -7,6 +7,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <initializer_list>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -145,6 +146,8 @@ class Comm {
   int ctas_for(uint64_t bytes, int cap, int per_cta_bytes) const;
   int nvls_ctas() const;
   void check_buf(const void* p, const char* what) const;
+  // the epilogue kernel of the unfused tails on r.T rows of an already reduced r.x
+  void launch_add_rmsnorm(const RmsNormArgs& r, int dtype, bool fp8, cudaStream_t stream);
   // host fake implementations (host_coll.cc)
   void host_barrier();
   void host_allreduce(const void* in, void* out, size_t count, int dtype, int op, float scale, int out_dtype);
@@ -184,6 +187,13 @@ void host_reduce_n(void* dst, const void* const* srcs, int n, size_t count, int 
 // CPU epilogue of allreduce_rmsnorm on an already reduced x (bf16 / fp16, fp32 arithmetic; e4m3 when out_scales)
 void host_add_rmsnorm(const void* x, const void* residual, void* residual_out, const void* weight, void* out,
                       float* out_scales, size_t T, size_t H, int dtype, float eps);
+// Checks of the fused residual add + RMSNorm layer tails (`op` names the call in messages): bf16 / fp16, H a multiple
+// of `mult` in [mult, max_h], H % 128 == 0 for the e4m3 output (fp8), T < 2^32; for T > 0 residual, residual_out,
+// weight, out (and out_scales with fp8) non-null; with `aligned` those, x and `extra` (optional inputs, may be null)
+// 16-byte aligned.  Returns the epilogue arguments (out_scales only with fp8).
+RmsNormArgs rmsnorm_tail_args(const char* op, void* x, const void* residual, void* residual_out, const void* weight,
+                              void* out, float* out_scales, int64_t T, int64_t H, int dtype, float eps, bool fp8,
+                              uint32_t max_h, uint32_t mult, bool aligned, std::initializer_list<const void*> extra = {});
 
 // torch.cuda.MemPool backend (mem_pool.cc): which communicator serves `uccl_b200_pool_malloc`
 void pool_install(std::shared_ptr<Comm> c);            // default for c->device()

@@ -270,8 +270,12 @@ uintptr_t EpBuffer::combine_input_ptr(int num_tokens, int hidden, int topk) {
   return (uintptr_t)(base_ + ctrl_bytes_ + (size_t)num_slots_ * arena_bytes_);
 }
 
-char* EpBuffer::stage_combine(const char* what, uintptr_t x, int num_recv, int H, int K, cudaStream_t st,
-                              EpCombineArgs& a) {
+namespace {
+int combine_grid(int num_sms) { return std::max(1, std::min(num_sms, kEpMaxBlocks)); }
+}  // namespace
+
+char* EpBuffer::stage_combine(const char* what, uintptr_t x, int num_recv, uintptr_t send_slot, uintptr_t bias0,
+                              uintptr_t bias1, int T, int H, int K, cudaStream_t st, EpCombineArgs& a) {
   UB_CHECK(H > 0 && H % 8 == 0, "%s: hidden (%d) must be a multiple of 8", what, H);
   UB_CHECK(K >= 0 && K <= kEpMaxTopk, "%s: bad num_topk %d", what, K);
   const int cap = combine_capacity_for(H, K);
@@ -291,6 +295,12 @@ char* EpBuffer::stage_combine(const char* what, uintptr_t x, int num_recv, int H
     a.x_off = comm_->heap_offset(arena);
   }
   a.topk_w_off = kNoOff;
+  a.send_slot = (const int32_t*)send_slot;
+  a.bias0 = (const void*)bias0;
+  a.bias1 = (const void*)bias1;
+  a.T = T;
+  a.H = H;
+  a.K = K;
   return arena;
 }
 
@@ -300,21 +310,15 @@ void EpBuffer::combine(uintptr_t x, int num_recv, uintptr_t topk_w, uintptr_t se
   UB_CHECK(send_slot != 0 && out != 0, "combine: handle/out missing");
   DevGuard g(comm_->device());
   EpCombineArgs a;
-  char* arena = stage_combine("combine", x, num_recv, H, K, st, a);
+  char* arena = stage_combine("combine", x, num_recv, send_slot, bias0, bias1, T, H, K, st, a);
   if (topk_w && out_topk_w && K > 0) {
     char* wdst = arena + align_up((size_t)combine_capacity_for(H, K) * H * 2, 256);
     UB_CUDA(cudaMemcpyAsync(wdst, (void*)topk_w, (size_t)num_recv * K * 4, cudaMemcpyDeviceToDevice, st));
     a.topk_w_off = comm_->heap_offset(wdst);
   }
-  a.send_slot = (const int32_t*)send_slot;
-  a.bias0 = (const void*)bias0;
-  a.bias1 = (const void*)bias1;
   a.out = (void*)out;
   a.out_topk_w = (float*)out_topk_w;
-  a.T = T;
-  a.H = H;
-  a.K = K;
-  int grid = std::max(1, std::min(num_sms, kEpMaxBlocks));
+  const int grid = combine_grid(num_sms);
   a.stages = st_comb_;
   const bool tma = pick_impl(grid, true) == EP_IMPL_TMA && ep_combine_tma_supported(a);
   last_comb_impl_ = tma ? EP_IMPL_TMA : EP_IMPL_REG;
@@ -326,35 +330,15 @@ void EpBuffer::combine(uintptr_t x, int num_recv, uintptr_t topk_w, uintptr_t se
 void EpBuffer::combine_rmsnorm(uintptr_t x, int num_recv, uintptr_t send_slot, uintptr_t bias0, uintptr_t bias1,
                                uintptr_t residual, uintptr_t residual_out, uintptr_t weight, uintptr_t out,
                                uintptr_t out_scales, int T, int H, float eps, int num_sms, cudaStream_t st) {
-  UB_CHECK(T >= 0, "combine_rmsnorm: bad token count %d", T);
   // a rank without tokens still joins the kernel's barriers; its (empty) tensors may have null pointers
-  UB_CHECK(T == 0 || (send_slot != 0 && residual != 0 && residual_out != 0 && weight != 0 && out != 0),
-           "combine_rmsnorm: handle, residual, residual_out, weight or out missing");
-  UB_CHECK(H >= 8 && (uint32_t)H <= kRmsMaxH, "combine_rmsnorm: hidden size %d must be a multiple of 8 in [8, %u]", H,
-           kRmsMaxH);
-  UB_CHECK(!out_scales || H % 128 == 0, "combine_rmsnorm: fp8 output needs hidden size %% 128 == 0 (got %d)", H);
-  UB_CHECK(((bias0 | bias1 | residual | residual_out | weight | out) & 15) == 0,
-           "combine_rmsnorm: bias, residual, residual_out, weight and out must be 16-byte aligned");
+  UB_CHECK(T == 0 || send_slot != 0, "combine_rmsnorm: handle missing");
+  const RmsNormArgs r = rmsnorm_tail_args("combine_rmsnorm", nullptr, (const void*)residual, (void*)residual_out,
+                                          (const void*)weight, (void*)out, (float*)out_scales, T, H, kBF16, eps,
+                                          out_scales != 0, kRmsMaxH, 8, true, {(const void*)bias0, (const void*)bias1});
   DevGuard g(comm_->device());
   EpCombineArgs a;
-  stage_combine("combine_rmsnorm", x, num_recv, H, 0, st, a);
-  a.send_slot = (const int32_t*)send_slot;
-  a.bias0 = (const void*)bias0;
-  a.bias1 = (const void*)bias1;
-  a.T = T;
-  a.H = H;
-  RmsNormArgs r;
-  memset(&r, 0, sizeof(r));
-  r.residual = (const void*)residual;
-  r.residual_out = (void*)residual_out;
-  r.weight = (const void*)weight;
-  r.out = (void*)out;
-  r.out_scales = (float*)out_scales;
-  r.T = (uint32_t)T;
-  r.H = (uint32_t)H;
-  r.eps = eps;
-  const int grid = std::max(1, std::min(num_sms, kEpMaxBlocks));
-  cudaError_t e = launch_ep_combine_rmsnorm(comm_->dev(), a, r, out_scales != 0, grid, st);
+  stage_combine("combine_rmsnorm", x, num_recv, send_slot, bias0, bias1, T, H, 0, st, a);
+  cudaError_t e = launch_ep_combine_rmsnorm(comm_->dev(), a, r, out_scales != 0, combine_grid(num_sms), st);
   UB_CHECK(e == cudaSuccess, "ep combine_rmsnorm launch failed: %s", cudaGetErrorString(e));
   ++launches_;
 }
@@ -488,8 +472,9 @@ uintptr_t EpBuffer::ll_combine_buffer(int buffer_idx, int H, int E, int M) const
   return (uintptr_t)(comm_->fabric().local() + l.comb_x_off);
 }
 
-uint64_t EpBuffer::ll_stage_combine(const char* what, uintptr_t x, int buffer_idx, int H, int E, int M,
-                                    cudaStream_t st, int phase, uintptr_t layout_range, bool use_logfmt) {
+EpLLCombineArgs EpBuffer::ll_combine_args(const char* what, uintptr_t x, int buffer_idx, uintptr_t topk_w,
+                                           uintptr_t send_pos, int T, int H, int K, int E, int M, cudaStream_t st,
+                                           int phase, uintptr_t layout_range, uintptr_t wait_stats, bool use_logfmt) {
   const int R = nranks();
   UB_CHECK(phase >= EP_LL_FULL && phase <= EP_LL_RECV, "%s: bad phase %d", what, phase);
   LLLayout l = ll_layout(buffer_idx, H, E, M);
@@ -518,26 +503,27 @@ uint64_t EpBuffer::ll_stage_combine(const char* what, uintptr_t x, int buffer_id
       UB_CUDA(cudaMemcpyAsync(arena, (void*)x, bytes, cudaMemcpyDeviceToDevice, st));
     }
   }
-  return l.comb_x_off;
+  EpLLCombineArgs a;
+  memset(&a, 0, sizeof(a));
+  a.x_off = l.comb_x_off;
+  a.send_pos = (const int64_t*)send_pos;
+  a.topk_weights = (const float*)topk_w;
+  a.T = T;
+  a.H = H;
+  a.K = K;
+  a.phase = phase;
+  a.wait_stats = (long long*)wait_stats;
+  return a;
 }
 
 void EpBuffer::ll_combine(uintptr_t x, int buffer_idx, uintptr_t topk_w, uintptr_t send_pos, uintptr_t out, int T,
                           int H, int K, int E, int M, int num_sms, cudaStream_t st, int phase, uintptr_t layout_range,
                           uintptr_t wait_stats, bool use_logfmt) {
   DevGuard g(comm_->device());
-  EpLLCombineArgs a;
-  memset(&a, 0, sizeof(a));
-  a.x_off = ll_stage_combine("ll_combine", x, buffer_idx, H, E, M, st, phase, layout_range, use_logfmt);
-  a.send_pos = (const int64_t*)send_pos;
-  a.topk_weights = (const float*)topk_w;
+  EpLLCombineArgs a = ll_combine_args("ll_combine", x, buffer_idx, topk_w, send_pos, T, H, K, E, M, st, phase,
+                                      layout_range, wait_stats, use_logfmt);
   a.out = (void*)out;
-  a.T = T;
-  a.H = H;
-  a.K = K;
-  a.phase = phase;
-  a.wait_stats = (long long*)wait_stats;
-  int grid = std::max(1, std::min(num_sms, kEpMaxBlocks));
-  cudaError_t e = launch_ep_ll_combine(comm_->dev(), a, grid, st);
+  cudaError_t e = launch_ep_ll_combine(comm_->dev(), a, combine_grid(num_sms), st);
   UB_CHECK(e == cudaSuccess, "ep ll_combine launch failed: %s", cudaGetErrorString(e));
   ++launches_;
 }
@@ -547,42 +533,21 @@ void EpBuffer::ll_combine_rmsnorm(uintptr_t x, int buffer_idx, uintptr_t topk_w,
                                   uintptr_t out_scales, int T, int H, int K, int E, int M, float eps, int num_sms,
                                   cudaStream_t st, int phase, uintptr_t layout_range, uintptr_t wait_stats,
                                   bool use_logfmt) {
-  UB_CHECK(T >= 0, "ll_combine_rmsnorm: bad token count %d", T);
   UB_CHECK(K > 0 && K <= 32, "ll_combine_rmsnorm: bad num_topk %d", K);
-  UB_CHECK(H > 0 && H % 128 == 0 && H <= 8192, "ll_combine_rmsnorm: hidden must be a multiple of 128 and <= 8192 (got %d)",
-           H);
   // a rank without tokens still joins the kernel's barriers; its (empty) tensors may have null pointers
-  UB_CHECK(T == 0 || (topk_w != 0 && send_pos != 0 && residual != 0 && residual_out != 0 && weight != 0 && out != 0),
-           "ll_combine_rmsnorm: topk_weights, send_pos, residual, residual_out, weight or out missing");
-  UB_CHECK(((shared | residual | residual_out | weight | out | out_scales) & 15) == 0,
-           "ll_combine_rmsnorm: shared, residual, residual_out, weight, out and scales must be 16-byte aligned");
+  UB_CHECK(T == 0 || (topk_w != 0 && send_pos != 0), "ll_combine_rmsnorm: topk_weights or send_pos missing");
+  const RmsNormArgs r = rmsnorm_tail_args("ll_combine_rmsnorm", nullptr, (const void*)residual, (void*)residual_out,
+                                          (const void*)weight, (void*)out, (float*)out_scales, T, H, kBF16, eps,
+                                          out_scales != 0, 8192, 128, true, {(const void*)shared});
   DevGuard g(comm_->device());
-  EpLLCombineArgs a;
-  memset(&a, 0, sizeof(a));
-  a.x_off = ll_stage_combine("ll_combine_rmsnorm", x, buffer_idx, H, E, M, st, phase, layout_range, use_logfmt);
-  a.send_pos = (const int64_t*)send_pos;
-  a.topk_weights = (const float*)topk_w;
-  a.T = T;
-  a.H = H;
-  a.K = K;
-  a.phase = phase;
-  a.wait_stats = (long long*)wait_stats;
-  const int grid = std::max(1, std::min(num_sms, kEpMaxBlocks));
+  const EpLLCombineArgs a = ll_combine_args("ll_combine_rmsnorm", x, buffer_idx, topk_w, send_pos, T, H, K, E, M, st,
+                                            phase, layout_range, wait_stats, use_logfmt);
+  const int grid = combine_grid(num_sms);
   cudaError_t e;
   if (phase == EP_LL_SEND) {
     // the pull design's send half only announces that the expert outputs are in place: the plain combine's
     e = launch_ep_ll_combine(comm_->dev(), a, grid, st);
   } else {
-    RmsNormArgs r;
-    memset(&r, 0, sizeof(r));
-    r.residual = (const void*)residual;
-    r.residual_out = (void*)residual_out;
-    r.weight = (const void*)weight;
-    r.out = (void*)out;
-    r.out_scales = (float*)out_scales;
-    r.T = (uint32_t)T;
-    r.H = (uint32_t)H;
-    r.eps = eps;
     e = launch_ep_ll_combine_rmsnorm(comm_->dev(), a, (const void*)shared, r, out_scales != 0, grid, st);
   }
   UB_CHECK(e == cudaSuccess, "ep ll_combine_rmsnorm launch failed: %s", cudaGetErrorString(e));

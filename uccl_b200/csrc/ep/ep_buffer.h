@@ -100,9 +100,11 @@ class EpBuffer {
 
  private:
   EpArena carve(int slot, int H, int mode, int K) const;
-  // checks of combine / combine_rmsnorm; zeroes `a` and sets a.x_off to the expert outputs every rank reads (x itself
-  // when it is the combine arena or symmetric, else a copy in the arena).  Returns the combine arena.
-  char* stage_combine(const char* what, uintptr_t x, int num_recv, int H, int K, cudaStream_t st, EpCombineArgs& a);
+  // checks of combine / combine_rmsnorm; zeroes `a`, sets the arguments both share and a.x_off to the expert outputs
+  // every rank reads (x itself when it is the combine arena or symmetric, else a copy in the arena).  Returns the
+  // combine arena.
+  char* stage_combine(const char* what, uintptr_t x, int num_recv, uintptr_t send_slot, uintptr_t bias0,
+                      uintptr_t bias1, int T, int H, int K, cudaStream_t st, EpCombineArgs& a);
   std::shared_ptr<Comm> comm_;
   char* base_ = nullptr;      // local VA of the EP block
   uint64_t base_off_ = 0;     // its heap offset
@@ -126,10 +128,11 @@ class EpBuffer {
     uint64_t cnt_tab_off, recv_x_off, recv_scales_off, recv_src_off, comb_x_off;
   };
   LLLayout ll_layout(int buffer_idx, int H, int E, int M) const;
-  // checks of ll_combine / ll_combine_rmsnorm, and (except in the RECV phase) the copy-in of an x that is not the
-  // LL combine buffer buffer_idx, or its in-place LogFMT pass.  Returns the heap offset of that buffer.
-  uint64_t ll_stage_combine(const char* what, uintptr_t x, int buffer_idx, int H, int E, int M, cudaStream_t st,
-                            int phase, uintptr_t layout_range, bool use_logfmt);
+  // checks and arguments (all but a.out) of ll_combine / ll_combine_rmsnorm, and (except in the RECV phase) the
+  // copy-in of an x that is not the LL combine buffer buffer_idx, or its in-place LogFMT pass
+  EpLLCombineArgs ll_combine_args(const char* what, uintptr_t x, int buffer_idx, uintptr_t topk_w, uintptr_t send_pos,
+                                  int T, int H, int K, int E, int M, cudaStream_t st, int phase,
+                                  uintptr_t layout_range, uintptr_t wait_stats, bool use_logfmt);
   char* ll_base_ = nullptr;
   size_t ll_bytes_ = 0;
   int ll_next_ = 0;

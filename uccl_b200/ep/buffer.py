@@ -21,7 +21,7 @@ from typing import List, Optional, Tuple, Union
 import torch
 
 from .. import _native
-from ..parallel.comm import Communicator, _overlaps
+from ..parallel.comm import Communicator, _rmsnorm_tail_args
 from .utils import EpHandle, EventHandle, EventOverlap
 
 RMS_MAX_HIDDEN = 16384  # kRmsMaxH: one 512-thread block holds a row in registers
@@ -29,44 +29,10 @@ LL_MAX_HIDDEN = 8192  # limit of the low-latency kernels
 LL_MAX_TOPK = 32
 
 
-def _rmsnorm_tail_args(name, x, T, H, residual, weight, extra, extra_name, residual_out, out, quant, device):
-    """Checks shared by the fused EP tails (``combine_rmsnorm``, ``low_latency_combine_rmsnorm``) on the CUDA and the
-    host backend, once ``x`` and ``H`` are checked: ``residual`` / ``weight``, the ``[T, H]`` inputs ``extra`` that are
-    added to the combined rows (``extra_name``: bias or shared), ``quant``, ``residual_out`` and ``out``, and that no
-    output overlaps an input.  Returns ``(residual_out, out, scales)`` with the defaults filled in (``scales`` is None
-    without fp8)."""
-    for t, nm in ((residual, "residual"), (weight, "weight")):
-        if t.dtype != torch.bfloat16 or not t.is_contiguous():
-            raise ValueError(f"uccl_b200.ep: {name} {nm} must be contiguous bf16")
-    if residual.shape != (T, H) or weight.shape != (H,):
-        raise ValueError(f"uccl_b200.ep: {name} needs residual [{T}, {H}] and weight [{H}] "
-                         f"(got {tuple(residual.shape)} and {tuple(weight.shape)})")
-    if quant not in (None, "fp8"):
-        raise ValueError(f"uccl_b200.ep: unsupported quant {quant!r} (None or 'fp8')")
-    fp8 = quant == "fp8"
-    if fp8 and H % 128:
-        raise ValueError(f"uccl_b200.ep: {name} fp8 output needs hidden size % 128 == 0 (got {H})")
-    for b in extra:
-        if b.dtype != torch.bfloat16 or b.shape != (T, H) or not b.is_contiguous():
-            raise ValueError(f"uccl_b200.ep: {name} {extra_name} must be contiguous bf16 [{T}, {H}]")
-    if residual_out is None:
-        residual_out = residual
-    if residual_out.dtype != torch.bfloat16 or residual_out.shape != (T, H) or not residual_out.is_contiguous():
-        raise ValueError(f"uccl_b200.ep: {name} residual_out must be contiguous bf16 [{T}, {H}]")
-    out_dtype = torch.float8_e4m3fn if fp8 else torch.bfloat16
-    if out is None:
-        out = torch.empty((T, H), dtype=out_dtype, device=device)
-    if out.dtype != out_dtype or out.shape != (T, H) or not out.is_contiguous():
-        raise ValueError(f"uccl_b200.ep: {name} out must be contiguous {out_dtype} [{T}, {H}]")
-    # peers read x while the kernel runs, and a row's residual and extra inputs are read before its outputs are stored
-    if any(_overlaps(out, t) for t in [x, residual, residual_out] + list(extra)):
-        raise ValueError(f"uccl_b200.ep: {name} out must not overlap x, residual, residual_out or {extra_name}")
-    if any(_overlaps(residual_out, t) for t in [x] + list(extra)) or (
-            residual_out.data_ptr() != residual.data_ptr() and _overlaps(residual_out, residual)):
-        raise ValueError(f"uccl_b200.ep: {name} residual_out must not overlap x, {extra_name} or residual "
-                         "(it may be residual itself)")
-    scales = torch.empty((T, H // 128), dtype=torch.float32, device=device) if fp8 else None
-    return residual_out, out, scales
+def _check_bf16_rows(name, what, ts, T, H):
+    for t in ts:
+        if t.dtype != torch.bfloat16 or t.shape != (T, H) or not t.is_contiguous():
+            raise ValueError(f"uccl_b200.ep: {name} {what} must be contiguous bf16 [{T}, {H}]")
 
 
 def _combine_rmsnorm_args(x, T, residual, weight, bias, residual_out, out, quant, device):
@@ -77,11 +43,14 @@ def _combine_rmsnorm_args(x, T, residual, weight, bias, residual_out, out, quant
     H = x.size(1)
     if H % 8 or not 8 <= H <= RMS_MAX_HIDDEN:
         raise ValueError(f"uccl_b200.ep: combine_rmsnorm hidden size {H} must be a multiple of 8 in [8, {RMS_MAX_HIDDEN}]")
+    if quant == "fp8" and H % 128:
+        raise ValueError(f"uccl_b200.ep: combine_rmsnorm fp8 output needs hidden size % 128 == 0 (got {H})")
     b0, b1 = bias if isinstance(bias, tuple) else (bias, None)
     biases = [b for b in (b0, b1) if b is not None]
-    residual_out, out, scales = _rmsnorm_tail_args("combine_rmsnorm", x, T, H, residual, weight, biases, "bias",
-                                                   residual_out, out, quant, device)
-    return b0, b1, residual_out, out, scales
+    _check_bf16_rows("combine_rmsnorm", "bias", biases, T, H)
+    # peers read x while the kernel runs, and a row's residual and biases are read before its outputs are stored
+    return (b0, b1) + _rmsnorm_tail_args("combine_rmsnorm", T, H, torch.bfloat16, device, residual, weight,
+                                         residual_out, out, quant, reads=[x] + biases)
 
 
 def _ll_combine_rmsnorm_args(x, topk_idx, topk_weights, R, M, H, E, residual, weight, shared, residual_out, out, quant,
@@ -102,8 +71,9 @@ def _ll_combine_rmsnorm_args(x, topk_idx, topk_weights, R, M, H, E, residual, we
         raise ValueError(f"uccl_b200.ep: {name} x must be contiguous bf16 [{E // R}, {R * M}, {H}] "
                          f"(got {x.dtype} {tuple(x.shape)})")
     extra = [shared] if shared is not None else []
-    return (T, K) + _rmsnorm_tail_args(name, x, T, H, residual, weight, extra, "shared", residual_out, out, quant,
-                                       device)
+    _check_bf16_rows(name, "shared", extra, T, H)
+    return (T, K) + _rmsnorm_tail_args(name, T, H, torch.bfloat16, device, residual, weight, residual_out, out, quant,
+                                       reads=[x] + extra)
 
 
 class Config:

@@ -129,26 +129,58 @@ class LowLatencyRuntime:
 
         hook = None
         if return_recv_hook:
-            sent = torch.cuda.Event()
-            sent.record(st)
-
-            def hook():
-                if self._pending is hook:
-                    self._pending = None
-                    with torch.cuda.device(dev):
-                        cur = torch.cuda.current_stream(dev)
-                        cur.wait_event(sent)  # the receive half reads the epoch the send half stored: order them even
-                        self.rt.ll_dispatch_recv(sms, stats_ptr, cur.cuda_stream)  # when the hook runs on another stream
-                        finish()
-
-            # everything the receive half touches stays alive until it has run
-            hook._keep = (x, topk_idx, recv_count, layout_range, send_pos, dispatch_wait_recv_cost_stats,
-                          cumulative_local_expert_recv_stats)
-            self._pending = hook
+            hook = self._recv_hook(st, lambda s: self.rt.ll_dispatch_recv(sms, stats_ptr, s),
+                                   (x, topk_idx, recv_count, layout_range, send_pos, dispatch_wait_recv_cost_stats,
+                                    cumulative_local_expert_recv_stats), finish)
         else:
             finish()
         ev = EventOverlap(EventHandle(st)) if async_finish else EventOverlap()
         return recv_x, recv_count, handle, ev, hook
+
+    def _recv_hook(self, st, recv, keep, finish=None):
+        """The hook of a SEND-phase call made on stream ``st``: ``recv(stream)`` launches the receive half on the stream
+        current when the hook runs, then ``finish()`` runs.  Everything the receive half touches (``keep``) stays alive
+        until it has run; the next low-latency call runs a hook that was never called."""
+        dev = self.buf.device
+        sent = torch.cuda.Event()
+        sent.record(st)
+
+        def hook():
+            if self._pending is hook:
+                self._pending = None
+                with torch.cuda.device(dev):
+                    cur = torch.cuda.current_stream(dev)
+                    cur.wait_event(sent)  # the receive half reads the epoch the send half stored: order them even
+                    recv(cur.cuda_stream)  # when the hook runs on another stream
+                    if finish is not None:
+                        finish()
+
+        hook._keep = keep
+        self._pending = hook
+        return hook
+
+    def _combine(self, launch, args, layout_range, stats, use_logfmt, async_finish, return_recv_hook, keep):
+        """Runs ``launch`` (``rt.ll_combine`` or ``rt.ll_combine_rmsnorm``) on ``args`` on the current stream: the whole
+        kernel, or with ``return_recv_hook`` the SEND half now and the RECV half from the returned hook.  Returns
+        ``(event, hook)``."""
+        assert not (async_finish and return_recv_hook), "async_finish and return_recv_hook are mutually exclusive"
+        b = self.buf
+        C = b._C
+        if stats is not None:
+            assert stats.dtype == torch.int64 and stats.numel() >= b.group_size
+        self._finish_pending()
+        st = torch.cuda.current_stream(b.device)
+        args = args + (self._sms(combine=True),)
+        kw = dict(layout_range=layout_range.data_ptr(), wait_stats=stats.data_ptr() if stats is not None else 0)
+        hook = None
+        if return_recv_hook:
+            # SEND half: (pack the expert outputs into the symmetric buffer and) announce that they are in place
+            launch(*args, st.cuda_stream, phase=C.EP_LL_SEND, use_logfmt=bool(use_logfmt), **kw)
+            hook = self._recv_hook(st, lambda s: launch(*args, s, phase=C.EP_LL_RECV, **kw),
+                                   keep + (layout_range, stats))
+        else:
+            launch(*args, st.cuda_stream, phase=C.EP_LL_FULL, use_logfmt=bool(use_logfmt), **kw)
+        return (EventOverlap(EventHandle(st)) if async_finish else EventOverlap()), hook
 
     def next_combine_buffer(self, handle):
         src_info, layout_range, M, H, E, idx, send_pos = handle
@@ -168,49 +200,15 @@ class LowLatencyRuntime:
                 raise ValueError("uccl_b200.ep: zero_copy and use_logfmt are mutually exclusive (as in the reference)")
             if x.shape[-1] % 128 != 0:
                 raise ValueError("uccl_b200.ep: use_logfmt needs hidden % 128 == 0")
-        assert not (async_finish and return_recv_hook), "async_finish and return_recv_hook are mutually exclusive"
-        self._finish_pending()
         src_info, layout_range, M, H, E, idx, send_pos = handle
-        b = self.buf
-        C = b._C
-        R = b.group_size
-        dev = b.device
         assert x.dtype == torch.bfloat16 and x.is_contiguous() and x.shape[-1] == H
         assert topk_weights.dtype == torch.float32 and topk_weights.is_contiguous()
         T, K = topk_weights.shape
-        st = torch.cuda.current_stream(dev)
         if out is None:
-            out = torch.empty((T, H), dtype=torch.bfloat16, device=dev)
-        if combine_wait_recv_cost_stats is not None:
-            assert combine_wait_recv_cost_stats.dtype == torch.int64 and combine_wait_recv_cost_stats.numel() >= R
-        stats_ptr = combine_wait_recv_cost_stats.data_ptr() if combine_wait_recv_cost_stats is not None else 0
-        sms = self._sms(combine=True)
-        args = (x.data_ptr(), idx, topk_weights.data_ptr(), send_pos.data_ptr(), out.data_ptr(), T, H, K, E, M, sms)
-        hook = None
-        if return_recv_hook:
-            # SEND half: (pack the expert outputs into the symmetric buffer and) announce that they are in place
-            self.rt.ll_combine(*args, st.cuda_stream, phase=C.EP_LL_SEND, layout_range=layout_range.data_ptr(),
-                               wait_stats=stats_ptr, use_logfmt=bool(use_logfmt))
-
-            sent = torch.cuda.Event()
-            sent.record(st)
-
-            def hook():
-                if self._pending is hook:
-                    self._pending = None
-                    with torch.cuda.device(dev):
-                        cur = torch.cuda.current_stream(dev)
-                        cur.wait_event(sent)  # see dispatch: epoch hand-over between the two halves
-                        self.rt.ll_combine(*args, cur.cuda_stream, phase=C.EP_LL_RECV,
-                                           layout_range=layout_range.data_ptr(), wait_stats=stats_ptr)
-
-            # alive until the receive half has run
-            hook._keep = (x, topk_weights, send_pos, out, layout_range, combine_wait_recv_cost_stats)
-            self._pending = hook
-        else:
-            self.rt.ll_combine(*args, st.cuda_stream, phase=C.EP_LL_FULL, layout_range=layout_range.data_ptr(),
-                               wait_stats=stats_ptr, use_logfmt=bool(use_logfmt))
-        ev = EventOverlap(EventHandle(st)) if async_finish else EventOverlap()
+            out = torch.empty((T, H), dtype=torch.bfloat16, device=self.buf.device)
+        args = (x.data_ptr(), idx, topk_weights.data_ptr(), send_pos.data_ptr(), out.data_ptr(), T, H, K, E, M)
+        ev, hook = self._combine(self.rt.ll_combine, args, layout_range, combine_wait_recv_cost_stats, use_logfmt,
+                                 async_finish, return_recv_hook, (x, topk_weights, send_pos, out))
         return out, ev, hook
 
     def combine_rmsnorm(self, x: torch.Tensor, topk_idx: torch.Tensor, topk_weights: torch.Tensor, handle,
@@ -225,51 +223,18 @@ class LowLatencyRuntime:
 
         if use_logfmt and zero_copy:
             raise ValueError("uccl_b200.ep: zero_copy and use_logfmt are mutually exclusive (as in the reference)")
-        assert not (async_finish and return_recv_hook), "async_finish and return_recv_hook are mutually exclusive"
         src_info, layout_range, M, H, E, idx, send_pos = handle
-        b = self.buf
-        C = b._C
-        R = b.group_size
-        dev = b.device
         T, K, residual_out, out, scales = _ll_combine_rmsnorm_args(
-            x, topk_idx, topk_weights, R, M, H, E, residual, weight, shared, residual_out, out, quant, dev)
+            x, topk_idx, topk_weights, self.buf.group_size, M, H, E, residual, weight, shared, residual_out, out, quant,
+            self.buf.device)
         if T > send_pos.size(0) or K != send_pos.size(1):
             raise ValueError(f"uccl_b200.ep: low_latency_combine_rmsnorm got topk_weights [{T}, {K}] for a dispatch of "
                              f"{tuple(send_pos.shape)}")
-        if combine_wait_recv_cost_stats is not None:
-            assert combine_wait_recv_cost_stats.dtype == torch.int64 and combine_wait_recv_cost_stats.numel() >= R
-        stats_ptr = combine_wait_recv_cost_stats.data_ptr() if combine_wait_recv_cost_stats is not None else 0
-        self._finish_pending()
-        st = torch.cuda.current_stream(dev)
-        sms = self._sms(combine=True)
         args = (x.data_ptr(), idx, topk_weights.data_ptr(), send_pos.data_ptr(),
                 shared.data_ptr() if shared is not None else 0, residual.data_ptr(), residual_out.data_ptr(),
                 weight.data_ptr(), out.data_ptr(), scales.data_ptr() if scales is not None else 0, T, H, K, E, M,
-                float(eps), sms)
-        hook = None
-        if return_recv_hook:
-            # SEND half: (pack the expert outputs into the symmetric buffer and) announce that they are in place
-            self.rt.ll_combine_rmsnorm(*args, st.cuda_stream, phase=C.EP_LL_SEND, layout_range=layout_range.data_ptr(),
-                                       wait_stats=stats_ptr, use_logfmt=bool(use_logfmt))
-
-            sent = torch.cuda.Event()
-            sent.record(st)
-
-            def hook():
-                if self._pending is hook:
-                    self._pending = None
-                    with torch.cuda.device(dev):
-                        cur = torch.cuda.current_stream(dev)
-                        cur.wait_event(sent)  # see dispatch: epoch hand-over between the two halves
-                        self.rt.ll_combine_rmsnorm(*args, cur.cuda_stream, phase=C.EP_LL_RECV,
-                                                   layout_range=layout_range.data_ptr(), wait_stats=stats_ptr)
-
-            # alive until the receive half has run
-            hook._keep = (x, topk_weights, send_pos, shared, residual, residual_out, weight, out, scales, layout_range,
-                          combine_wait_recv_cost_stats)
-            self._pending = hook
-        else:
-            self.rt.ll_combine_rmsnorm(*args, st.cuda_stream, phase=C.EP_LL_FULL, layout_range=layout_range.data_ptr(),
-                                       wait_stats=stats_ptr, use_logfmt=bool(use_logfmt))
-        ev = EventOverlap(EventHandle(st)) if async_finish else EventOverlap()
+                float(eps))
+        ev, hook = self._combine(self.rt.ll_combine_rmsnorm, args, layout_range, combine_wait_recv_cost_stats,
+                                 use_logfmt, async_finish, return_recv_hook,
+                                 (x, topk_weights, send_pos, shared, residual, residual_out, weight, out, scales))
         return ((out, scales) if scales is not None else out), ev, hook

@@ -79,6 +79,41 @@ def _overlaps(a: torch.Tensor, b: torch.Tensor) -> bool:
     return a.device == b.device and a0 < b1 and b0 < a1
 
 
+def _rmsnorm_tail_args(op, rows, H, dtype, device, residual, weight, residual_out, out, quant, reads=(), writes=()):
+    """Checks and defaults of the fused residual add + RMSNorm layer tails, once ``op`` has checked its own inputs.
+
+    ``residual``, ``residual_out`` (default: ``residual``) and ``out`` (default: a fresh tensor) are contiguous
+    ``[rows, H]``, ``weight`` is ``[H]``, all of ``dtype`` except an e4m3 ``out`` with ``quant="fp8"``.  A tensor the op
+    writes (``residual_out``, ``out`` and ``writes``) must not overlap another operand (those, ``residual`` and
+    ``reads``); only ``residual_out`` may be ``residual`` itself.  ``weight`` is read-only and never conflicts.
+    Returns ``(residual_out, out, scales)``; ``scales`` is fp32 ``[rows, H / 128]`` with fp8, else None."""
+    if quant not in (None, "fp8"):
+        raise ValueError(f"uccl_b200: {op}: unsupported quant {quant!r} (None or 'fp8')")
+    fp8 = quant == "fp8"
+    out_dtype = torch.float8_e4m3fn if fp8 else dtype
+    if residual_out is None:
+        residual_out = residual
+    if out is None:
+        out = torch.empty((rows, H), dtype=out_dtype, device=device)
+    for t, name, shape, dt in ((residual, "residual", (rows, H), dtype), (weight, "weight", (H,), dtype),
+                               (residual_out, "residual_out", (rows, H), dtype), (out, "out", (rows, H), out_dtype)):
+        if t.dtype != dt or t.shape != shape or not t.is_contiguous():
+            raise ValueError(f"uccl_b200: {op} {name} must be contiguous {dt} {list(shape)} "
+                             f"(got {t.dtype} {list(t.shape)})")
+    written = [residual_out, out, *writes]
+    operands = written + [residual, *reads]
+    for i, w in enumerate(written):
+        for j in range(i + 1, len(operands)):
+            o = operands[j]
+            if i == 0 and j == len(written) and w.data_ptr() == o.data_ptr():
+                continue  # residual_out is residual itself
+            if _overlaps(w, o):
+                raise ValueError(f"uccl_b200: {op} outputs must not overlap each other or an input "
+                                 "(residual_out may be residual itself)")
+    scales = torch.empty((rows, H // 128), dtype=torch.float32, device=device) if fp8 else None
+    return residual_out, out, scales
+
+
 class _HeapBlock:
     """Owns one symmetric-heap allocation; exposes it to torch without copying."""
 
@@ -262,34 +297,13 @@ class Communicator:
         (small decode batches) everything is one kernel; larger ones run the selected all-reduce and then one
         epilogue kernel.  Both paths give bitwise identical results on every rank.  The fp8 output is the
         ``(x, scales)`` format of ``ep.utils.per_token_cast_to_fp8`` and ``ep.Buffer.dispatch``."""
-        for t, name in ((x, "x"), (residual, "residual"), (weight, "weight")):
-            self._check(t, name)
+        self._check(x, "x")
         if x.dim() != 2:
             raise ValueError("uccl_b200: all_reduce_rmsnorm x must be [tokens, hidden]")
         T, H = x.shape
-        if residual.shape != x.shape or weight.shape != (H,) or residual.dtype != x.dtype or weight.dtype != x.dtype:
-            raise ValueError("uccl_b200: all_reduce_rmsnorm needs residual [T, H] and weight [H] of x's dtype")
-        if quant not in (None, "fp8"):
-            raise ValueError(f"uccl_b200: unsupported quant {quant!r} (None or 'fp8')")
-        if residual_out is None:
-            residual_out = residual
-        self._check(residual_out, "residual_out")
-        if residual_out.shape != x.shape or residual_out.dtype != x.dtype:
-            raise ValueError("uccl_b200: all_reduce_rmsnorm residual_out must match x")
-        fp8 = quant == "fp8"
-        out_dtype = torch.float8_e4m3fn if fp8 else x.dtype
-        if out is None:
-            out = torch.empty((T, H), dtype=out_dtype, device=x.device)
-        self._check(out, "out")
-        if out.shape != x.shape or out.dtype != out_dtype:
-            raise ValueError(f"uccl_b200: all_reduce_rmsnorm out must be [T, H] of {out_dtype}")
-        scales = torch.empty((T, H // 128), dtype=torch.float32, device=x.device) if fp8 else None
-        if _overlaps(out, x) or _overlaps(out, residual):
-            raise ValueError("uccl_b200: all_reduce_rmsnorm out must not alias x or residual")
-        if _overlaps(x, residual) or _overlaps(residual_out, x) or _overlaps(residual_out, out) or (
-                residual_out.data_ptr() != residual.data_ptr() and _overlaps(residual_out, residual)):
-            raise ValueError("uccl_b200: all_reduce_rmsnorm x, residual and residual_out must not overlap "
-                             "(residual_out may be residual itself)")
+        residual_out, out, scales = _rmsnorm_tail_args("all_reduce_rmsnorm", T, H, x.dtype, x.device, residual, weight,
+                                                       residual_out, out, quant, writes=(x,))
+        fp8 = scales is not None
         a = ALGOS[algo] if isinstance(algo, str) else int(algo)
         self._c.allreduce_rmsnorm(x.data_ptr(), residual.data_ptr(), residual_out.data_ptr(), weight.data_ptr(),
                                   out.data_ptr(), scales.data_ptr() if fp8 else 0, T, H, dtype_code(x.dtype),
@@ -315,39 +329,16 @@ class Communicator:
         ``x`` and the full residual.  The fp8 output is the ``(x, scales)`` format of
         ``ep.utils.per_token_cast_to_fp8``; the full ``[T, H]`` pair for the next column-parallel layer is two plain
         :meth:`all_gather` calls, one of ``out_e4m3`` and one of ``scales``."""
-        for t, name in ((x, "x"), (residual, "residual"), (weight, "weight")):
-            self._check(t, name)
+        self._check(x, "x")
         if x.dim() != 2:
             raise ValueError("uccl_b200: reduce_scatter_rmsnorm x must be [tokens, hidden]")
         T, H = x.shape
         n = self.world_size
         if T % n:
             raise ValueError(f"uccl_b200: reduce_scatter_rmsnorm needs tokens ({T}) divisible by the world size ({n})")
-        Tl = T // n
-        if residual.shape != (Tl, H) or weight.shape != (H,) or residual.dtype != x.dtype or weight.dtype != x.dtype:
-            raise ValueError("uccl_b200: reduce_scatter_rmsnorm needs residual [T / world_size, H] and weight [H] "
-                             "of x's dtype")
-        if quant not in (None, "fp8"):
-            raise ValueError(f"uccl_b200: unsupported quant {quant!r} (None or 'fp8')")
-        if residual_out is None:
-            residual_out = residual
-        self._check(residual_out, "residual_out")
-        if residual_out.shape != (Tl, H) or residual_out.dtype != x.dtype:
-            raise ValueError("uccl_b200: reduce_scatter_rmsnorm residual_out must match residual")
-        fp8 = quant == "fp8"
-        out_dtype = torch.float8_e4m3fn if fp8 else x.dtype
-        if out is None:
-            out = torch.empty((Tl, H), dtype=out_dtype, device=x.device)
-        self._check(out, "out")
-        if out.shape != (Tl, H) or out.dtype != out_dtype:
-            raise ValueError(f"uccl_b200: reduce_scatter_rmsnorm out must be [T / world_size, H] of {out_dtype}")
-        scales = torch.empty((Tl, H // 128), dtype=torch.float32, device=x.device) if fp8 else None
-        if _overlaps(out, x) or _overlaps(out, residual):
-            raise ValueError("uccl_b200: reduce_scatter_rmsnorm out must not alias x or residual")
-        if _overlaps(x, residual) or _overlaps(residual_out, x) or _overlaps(residual_out, out) or (
-                residual_out.data_ptr() != residual.data_ptr() and _overlaps(residual_out, residual)):
-            raise ValueError("uccl_b200: reduce_scatter_rmsnorm x, residual and residual_out must not overlap "
-                             "(residual_out may be residual itself)")
+        residual_out, out, scales = _rmsnorm_tail_args("reduce_scatter_rmsnorm", T // n, H, x.dtype, x.device, residual,
+                                                       weight, residual_out, out, quant, writes=(x,))
+        fp8 = scales is not None
         self._c.reduce_scatter_rmsnorm(x.data_ptr(), residual.data_ptr(), residual_out.data_ptr(), weight.data_ptr(),
                                        out.data_ptr(), scales.data_ptr() if fp8 else 0, T, H, dtype_code(x.dtype),
                                        float(eps), int(fp8), self._stream(stream))
